@@ -104,6 +104,7 @@ struct lk_context {
     DevBuf ins_pts, ins_root, ins_pend, ins_touched, ins_counters, ins_list;
     uint64_t ins_pend_nodes = 0;
     int trace_on = 0;
+    uint32_t trace_seq = 0;  // fused launches traced since the trace was switched on or last read back
     int lane_cache = 1;
     int use_fused = 1;      // batch-of-one runs go through the persistent per-scan kernel
     FusedInline inl;         // parameter-block image of the small inputs (direct mode)
@@ -193,6 +194,11 @@ void fill_globals(lk_context* c, const double* extR, const double* extT) {
     g.max_points_num = c->mc.max_points_num;
     for (int i = 0; i < 5; ++i) g.layer_init_num[i] = c->mc.layer_init_num[i];
 }
+
+// the trace buffer ((1 << 16) * 8 doubles' worth of %globaltimer stamps): TRACE_AREAS areas of TRACE_AREA stamps, one per
+// traced fused launch (a launch writes 32 per block plus, streaming with the insert inside, 64 x 8 per-bucket stamps)
+constexpr size_t TRACE_AREA = 8192;
+constexpr size_t TRACE_AREAS = 64;
 
 // Chunking is a function of the bucket and of the kernel family alone, so results are bitwise independent
 // of how a batch is sharded across GPUs (SURVEY §4 multi-GPU invariant).
@@ -385,6 +391,7 @@ int lk_set_param(lk_handle h, const char* name, double value) {
             LK_CUDA(h, h->trace.ensure((size_t)(1 << 16) * 8 * 8));
             LK_CUDA(h, cudaMemset(h->trace.p, 0, (size_t)(1 << 16) * 8 * 8));
         }
+        h->trace_seq = 0;
         return LK_OK;
     }
     return fail(h, LK_ERR_INVALID_ARG, std::string("unknown parameter ") + name);
@@ -401,6 +408,7 @@ int lk_debug_read(lk_handle h, int what, void* dst, size_t bytes) {
     cudaSetDevice(h->device);
     h->prev_fused = false;
     DevBuf* b = what == 0 ? &h->partial : (what == 1 ? &h->sc : &h->trace);
+    if (what == 2) h->trace_seq = 0;
     if (bytes > b->cap) bytes = b->cap;
     LK_CUDA(h, cudaMemcpy(dst, b->p, bytes, cudaMemcpyDeviceToHost));
     return LK_OK;
@@ -900,7 +908,9 @@ static int run_range_impl(lk_handle h, uint32_t first, uint32_t count, int iters
             fa.acc_norm = mq->acc_norm;
         }
         fa.ecfg = h->ec;
-        fa.trace = h->trace_on ? h->trace.as<unsigned long long>() : nullptr;
+        // back-to-back launches trace into consecutive areas (TRACE_AREA stamps each, TRACE_AREAS of them, cycling), so the
+        // overlap of one launch with the next can be read back; the first launch after lk_debug_read starts again at area 0
+        fa.trace = h->trace_on ? h->trace.as<unsigned long long>() + (size_t)(h->trace_seq++ % TRACE_AREAS) * TRACE_AREA : nullptr;
         fa.g = h->g;
         if (update_map) {
             fa.insert = 1;

@@ -38,6 +38,9 @@ __device__ __forceinline__ unsigned long long gtime() {
     return t;
 }
 #define FT(slot) do { if (a.trace && threadIdx.x == 0 && (slot) < 32) a.trace[(size_t)blockIdx.x * 32 + (slot)] = gtime(); } while (0)
+// per-iteration stamps of the first three exchanges i: 14 + i pass done, 2 + 4i block row in shared memory, 3 + 4i all-reduce
+// total in shared memory, 4 + 4i solve done (tools/trace_fused.py)
+#define FTI(slot) do { if (it_global < 3) FT(slot); } while (0)
 // per-bucket stamps of the streaming variants (block 0, first 64 buckets, 8 stamps each, behind the per-block area)
 #define FTS(slot) do { if (a.trace && blockIdx.x == 0 && threadIdx.x == 0 && k < 64) a.trace[(size_t)gridDim.x * 32 + (size_t)k * 8 + (slot)] = gtime(); } while (0)
 
@@ -219,10 +222,11 @@ __global__ void __launch_bounds__(BLOCK, 1) k_scan_fused(const __grid_constant__
             for (int i = 0; i < 32; ++i) acc[i] = 0.0;
             if (!a.lane_cache && lc.have == 2) lc.have = 1;
             cached_points_pass<BLOCK, INS>(&sm->u.pass, phase, my_count, sm->sc, a.mv, a.g, acc, lc, pre);
+            FTI(14 + it_global);
             const double tot = warp_transpose_sum(acc, lane);
             sm->slice[warp * 32 + lane] = tot;
             __syncthreads();
-            FT(2 + it_global * 4);
+            FTI(2 + it_global * 4);
             if (it == 0) FTS(3);
             // 2) all-reduce of the block rows (warp 0), no barrier
             if (warp == 0) {
@@ -234,13 +238,13 @@ __global__ void __launch_bounds__(BLOCK, 1) k_scan_fused(const __grid_constant__
             }
             dep_waited = true;
             __syncthreads();
-            FT(3 + it_global * 4);
+            FTI(3 + it_global * 4);
             if (it == 0) FTS(4);
             // 3) every block solves redundantly (eskf.cc:91-113); the covariance update of the last iteration is
             //    deferred behind the re-projection, and skipped where nobody reads the result
             const bool last = it == a.iters - 1;
             const uint32_t n = block_solve_state(&sm->f);
-            FT(4 + it_global * 4);
+            FTI(4 + it_global * 4);
             if (n > 0) {
                 updated = true;
                 if (tid == 0) sm->clk[1] = in.t_bucket;  // KILO.cc:212
@@ -261,6 +265,7 @@ __global__ void __launch_bounds__(BLOCK, 1) k_scan_fused(const __grid_constant__
                 o.w = updated ? 255.0f : 0.0f;
                 a.world[my_start + tid] = o;
             }
+            FT(20);
             if (cov_pending) block_cov_update<BLOCK>(&sm->f);
         } else {
             // 4') re-projection AND map insert with the updated state and covariance (KILO.cc:216-231). Phase 1, the blocks

@@ -234,19 +234,27 @@ __device__ __forceinline__ bool point_row(float4 pt, const ScanConst& sc, const 
     return ok;
 }
 
+// One exchange step of warp_transpose_sum. The offset must be a compile-time constant: a loop over halving offsets has no
+// trip count the compiler can find, stays rolled, and the array it indexes then lives in local memory.
+template <int OFF>
+__device__ __forceinline__ void warp_transpose_step(double (&v)[32], int lane) {
+    const bool upper = (lane & OFF) != 0;
+#pragma unroll
+    for (int i = 0; i < OFF; ++i) {
+        double send = upper ? v[i] : v[i + OFF];
+        double keep = upper ? v[i + OFF] : v[i];
+        v[i] = keep + __shfl_xor_sync(0xffffffffu, send, OFF);
+    }
+}
+
 // Sum of 32 per-lane values over the warp with value/lane transposition: after the 5 exchange
 // steps lane L holds the warp total of value L (31 exchanges instead of 32 x 5 shuffles).
 __device__ __forceinline__ double warp_transpose_sum(double (&v)[32], int lane) {
-#pragma unroll
-    for (int off = 16; off >= 1; off >>= 1) {
-        const bool upper = (lane & off) != 0;
-#pragma unroll
-        for (int i = 0; i < off; ++i) {
-            double send = upper ? v[i] : v[i + off];
-            double keep = upper ? v[i + off] : v[i];
-            v[i] = keep + __shfl_xor_sync(0xffffffffu, send, off);
-        }
-    }
+    warp_transpose_step<16>(v, lane);
+    warp_transpose_step<8>(v, lane);
+    warp_transpose_step<4>(v, lane);
+    warp_transpose_step<2>(v, lane);
+    warp_transpose_step<1>(v, lane);
     return v[0];
 }
 

@@ -1,34 +1,118 @@
-"""Per-phase %globaltimer trace of the fused per-scan kernel (latency diagnosis)."""
-import sys, os, numpy as np
-ROOT=os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-for p in ("leg-kilo_b200/python","tests"): sys.path.insert(0, os.path.join(ROOT,p))
+"""Per-phase %globaltimer trace of the fused per-scan kernel at the headline shape (latency diagnosis).
+
+  python tools/trace_fused.py [--workload leg_fusion_b1] [--scans 512] [--launches 48] [name=value ...]
+
+Builds bench.py's workload (by default leg_fusion_b1 with its 512-scan ring: inputs larger than L2), warms the ring up
+once, then issues --launches back-to-back launches exactly as bench.py does (kernel_timing = 0, so consecutive launches
+overlap through programmatic dependent launch). Only those launches carry stamps; each writes its own trace area. The
+first of them follows the switch that turns tracing on and is launched without PDL, so it is left out of the figures.
+Stamps per block (slots, see lk_fused.cu): 0 entry, 1 first pass starts, per iteration i 14+i pass done,
+2+4i block row in shared memory, 3+4i all-reduce total in hand, 4+4i solve done, 20 re-projection stored, 30 loop left,
+31 end; a build without the pass-done and re-projection stamps gets the combined phases printed instead. Times in
+microseconds: medians over the traced launches (min and max beside them) of per-launch medians over blocks, unless the
+name says "slowest block" or "last block".
+"""
+import argparse
+import os
+import sys
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+for p in ("leg-kilo_b200/python", "tests"):
+    sys.path.insert(0, os.path.join(ROOT, p))
 sys.path.insert(0, ROOT)
-import bench
-from legkilo_b200 import Engine, abi, lib, _p
-name = sys.argv[1] if len(sys.argv) > 1 else "small"
-w = bench.WORKLOADS[name]; ring = 16 if name == "small" else 128
-wl = bench.build_workload(w, 0, ring); cfg = wl["cfg"]
-eng = Engine(cfg); eng.map_build(wl["map_world"], wl["map_body"])
-CL = True
-for kv in sys.argv[2:]:
-    k, v = kv.split("="); eng.set_param(k, float(v))
-    if k == "cluster" and float(v) == 0: CL = False
-eng.stage(wl["x0"], abi.init_cov(ring), abi.process_cov_Q(cfg), np.zeros(ring, abi.CLOCK_DTYPE), wl["pts"], wl["offs"], np.zeros(ring))
-for i in range(ring * 2): eng.run_range(i % ring, 1, iters=3)
-eng.sync(); eng.set_param("trace", 1)
-us = lambda v: v / 1e3
-for scan in (3, 4, 5):
-    eng.run_range(scan, 1, iters=3); eng.sync()
-    tr = np.zeros((1 << 16) * 8, np.uint64); lib().lk_debug_read(eng.h, 2, _p(tr), tr.nbytes)
-    nb = int((wl["offs"][scan + 1] - wl["offs"][scan] + 255) // 256)
-    nbg = nb
-    b = tr[:nb * 32].reshape(nb, 32).astype(np.int64); t0 = b[:, 0].min()
-    print("scan %d (%d blocks): start spread %.2f, load filter + init %.2f" % (scan, nb, us(b[:, 0].max() - t0), us(np.median(b[:, 1] - b[:, 0]))))
-    prev = b[:, 1]
-    for it in range(3):
-        pts = b[:, 2 + 4 * it] - prev; ar = b[:, 3 + 4 * it] - b[:, 2 + 4 * it]; sol = b[:, 4 + 4 * it] - b[:, 3 + 4 * it]
-        last_in = b[:, 2 + 4 * it].max()
-        print("  it%d: points med %.2f max %.2f (last block in at %.2f) | all-reduce wait med %.2f, done %.2f after the last block (at %.2f) | solve %.2f" % (
-            it, us(np.median(pts)), us(pts.max()), us(last_in - t0), us(np.median(ar)), us(np.median(b[:, 3 + 4 * it]) - last_in), us(np.median(b[:, 3 + 4 * it]) - t0), us(np.median(sol))))
-        prev = b[:, 4 + 4 * it]
-    print("  reproject (+cov on block 0) med %.2f, block 0 %.2f; end at med %.2f max %.2f us" % (us(np.median(b[:, 30] - prev)), us(b[0, 30] - prev[0]), us(np.median(b[:, 31]) - t0), us(b[:, 31].max() - t0)))
+import bench  # noqa: E402
+from legkilo_b200 import Engine, _p, abi, lib  # noqa: E402
+
+TRACE_AREA, TRACE_AREAS = 8192, 64  # lk_api.cu
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--workload", default="leg_fusion_b1")
+    ap.add_argument("--scans", type=int, default=0, help="ring size (default: bench.py's)")
+    ap.add_argument("--launches", type=int, default=48)
+    ap.add_argument("param", nargs="*", help="engine parameter name=value (lk_set_param)")
+    args = ap.parse_args()
+    L = min(args.launches, TRACE_AREAS)
+    w = bench.WORKLOADS[args.workload]
+    assert w["batch"] == 1, "the fused kernel runs batch-of-one workloads"
+    ring = args.scans or w["ring"]
+    wl = bench.build_workload(w, 0, ring)
+    cfg = wl["cfg"]
+    eng = Engine(cfg)
+    for kv in args.param:
+        k, v = kv.split("=")
+        eng.set_param(k, float(v))
+    eng.set_param("kernel_timing", 0)
+    eng.map_build(wl["map_world"], wl["map_body"])
+    eng.stage(wl["x0"], abi.init_cov(ring), abi.process_cov_Q(cfg), np.zeros(ring, abi.CLOCK_DTYPE), wl["pts"], wl["offs"],
+              np.zeros(ring))
+    for i in range(ring):
+        eng.run_range(i, 1, iters=w["iters"])
+    eng.sync()
+    eng.set_param("trace", 1)
+    scans = [(ring // 2 + i) % ring for i in range(L)]
+    for s in scans:
+        eng.run_range(s, 1, iters=w["iters"])
+    eng.sync()
+    tr = np.zeros(TRACE_AREA * TRACE_AREAS, np.uint64)
+    lib().lk_debug_read(eng.h, 2, _p(tr), tr.nbytes)
+    eng.set_param("trace", 0)
+    offs = wl["offs"]
+    T = []
+    for j, s in enumerate(scans):
+        nb = int((offs[s + 1] - offs[s] + 255) // 256)
+        T.append(tr[j * TRACE_AREA: j * TRACE_AREA + nb * 32].reshape(nb, 32).astype(np.int64))
+    it_n = w["iters"]
+    us = 1e-3
+
+    def has(b, k):
+        return bool((b[:, k] != 0).all())
+
+    rows = {}
+
+    def put(name, v):
+        rows.setdefault(name, []).append(v)
+
+    for j in range(1, L):
+        b = T[j]
+        t0 = b[:, 0].min()
+        put("launch: block start spread", (b[:, 0].max() - t0) * us)
+        put("prologue (entry -> first pass)", np.median(b[:, 1] - b[:, 0]) * us)
+        prev = b[:, 1]
+        for it in range(it_n):
+            s_row, s_ar, s_sol, s_pass = 2 + 4 * it, 3 + 4 * it, 4 + 4 * it, 14 + it
+            if has(b, s_pass):
+                put("it%d pass" % it, np.median(b[:, s_pass] - prev) * us)
+                put("it%d reduction -> row in smem" % it, np.median(b[:, s_row] - b[:, s_pass]) * us)
+            else:
+                put("it%d pass + reduction" % it, np.median(b[:, s_row] - prev) * us)
+            put("it%d pass: slowest block" % it, (b[:, s_row] - prev).max() * us)
+            last_in = b[:, s_row].max()
+            put("it%d all-reduce: wait" % it, np.median(b[:, s_ar] - b[:, s_row]) * us)
+            put("it%d all-reduce: done after last block row" % it, (np.median(b[:, s_ar]) - last_in) * us)
+            put("it%d solve (-> next pass)" % it, np.median(b[:, s_sol] - b[:, s_ar]) * us)
+            prev = b[:, s_sol]
+        if has(b, 20):
+            put("re-projection", np.median(b[:, 20] - prev) * us)
+            put("after re-projection -> loop left", np.median(b[:, 30] - b[:, 20]) * us)
+        else:
+            put("re-projection (+ cov)", np.median(b[:, 30] - prev) * us)
+        put("block 0 tail (cov update, P store)", (b[0, 31] - b[0, 30]) * us)
+        put("launch span (first entry -> last end)", (b[:, 31].max() - t0) * us)
+        if j + 1 < L:
+            n = T[j + 1]
+            put("next launch: first block entry - this launch's last end", (n[:, 0].min() - b[:, 31].max()) * us)
+            put("next launch: first exchange done - this launch's last end", (n[:, 3].min() - b[:, 31].max()) * us)
+            put("period (first entry to next first entry)", (n[:, 0].min() - t0) * us)
+    nbs = sorted({t.shape[0] for t in T})
+    print("%s, ring %d, %d traced launches (%d..%d blocks), %s" % (args.workload, ring, L - 1, nbs[0], nbs[-1], bench.gpu_identity(0)))
+    for k, v in rows.items():
+        v = np.asarray(v)
+        print("  %-60s %8.2f  (min %.2f, max %.2f)" % (k, np.median(v), v.min(), v.max()))
+
+
+if __name__ == "__main__":
+    main()
