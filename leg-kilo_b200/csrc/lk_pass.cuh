@@ -305,10 +305,13 @@ struct LaneCache {
 template <int NTHREADS>
 struct CachedPassSmem {
     __align__(16) unsigned char tile[2][NTHREADS * TILE_STRIDE];  // [0] home records, [1] neighbour records
+    // Every lane's point context of the current pass. The evaluations read it from here and the descent receives its
+    // address, so it never lives in the stack frame (which the L1 left beside this much shared memory cannot hold: every
+    // access would go to L2); the fallback round reads the failing lane's context in place, without a copy.
+    PointCtx pt[NTHREADS];
     struct __align__(8) Fallback {
-        double pc[11];
         int near;
-        uint32_t idx;
+        uint32_t idx;  // the failing lane: its context is pt[idx], its neighbour record tile[1] slot idx
     } fb[NTHREADS];
     uint64_t bar[NTHREADS / 32];
     uint32_t wcnt[NTHREADS / 32];
@@ -328,7 +331,7 @@ __device__ __forceinline__ void cached_points_pass(CachedPassSmem<NTHREADS>* ps,
                                                    double (&acc)[32], LaneCache& lc, float4 pre) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const bool active = (uint32_t)tid < count;
-    PointCtx pc;
+    PointCtx& pc = ps->pt[tid];
     int root = -1, near = -1;
     bool gather_home = false, gather_near = false;
     if (active) {
@@ -399,20 +402,26 @@ __device__ __forceinline__ void cached_points_pass(CachedPassSmem<NTHREADS>* ps,
         plane_from_smem(home_slot, r);
         ok = eval_record<COH>(mv.nodes, r, pc, sc, g, row);
     }
-    fallback_list<NTHREADS>(ps, root >= 0 && !ok && near >= 0, pc, near, lane, warp);
+    {  // the failing points, listed per warp in lane order as fallback_list does; their contexts stay in pt
+        const bool want = root >= 0 && !ok && near >= 0;
+        const uint32_t m = __ballot_sync(0xffffffffu, want);
+        if (lane == 0) ps->wcnt[warp] = (uint32_t)__popc(m);
+        if (want) {
+            auto& f = ps->fb[(uint32_t)warp * 32u + (uint32_t)__popc(m & ((1u << lane) - 1u))];
+            f.near = near;
+            f.idx = (uint32_t)tid;
+        }
+    }
     __syncthreads();
     // ---- fallback round: the neighbour voxel of the points that failed at home, record already staged -------
     uint32_t fb_slot = 0;
     Row row2;
     bool ok2 = false;
     if (fallback_pick<NTHREADS>(ps, fb_slot)) {
-        const typename CachedPassSmem<NTHREADS>::Fallback& f = ps->fb[fb_slot];
-        PointCtx fc;
-        fc.pbx = f.pc[0]; fc.pby = f.pc[1]; fc.pbz = f.pc[2]; fc.pix = f.pc[3]; fc.piy = f.pc[4]; fc.piz = f.pc[5];
-        fc.pwx = f.pc[6]; fc.pwy = f.pc[7]; fc.pwz = f.pc[8]; fc.r2 = f.pc[9]; fc.range2 = f.pc[10];
+        const uint32_t idx = ps->fb[fb_slot].idx;
         PlaneRec r;
-        plane_from_smem(ps->tile[1] + (size_t)f.idx * TILE_STRIDE, r);
-        ok2 = eval_record<COH>(mv.nodes, r, fc, sc, g, row2);
+        plane_from_smem(ps->tile[1] + (size_t)idx * TILE_STRIDE, r);
+        ok2 = eval_record<COH>(mv.nodes, r, ps->pt[idx], sc, g, row2);
     }
     if (ok) accumulate_row(row, acc);
     if (ok2) accumulate_row(row2, acc);

@@ -117,8 +117,12 @@ __device__ __forceinline__ uint32_t block_solve_state(BlockFilter* f, unsigned l
             if (lane < 9) {
                 double E[9];
                 so3_exp3(d0, d1, d2, E);
+                // column j of E picked with compile-time indices: E indexed at run time would live in local memory
                 const int i = lane / 3, j = lane % 3;
-                rv = f->x[i * 3] * E[j] + f->x[i * 3 + 1] * E[3 + j] + f->x[i * 3 + 2] * E[6 + j];
+                const double e0 = j == 0 ? E[0] : (j == 1 ? E[1] : E[2]);
+                const double e1 = j == 0 ? E[3] : (j == 1 ? E[4] : E[5]);
+                const double e2 = j == 0 ? E[6] : (j == 1 ? E[7] : E[8]);
+                rv = f->x[i * 3] * e0 + f->x[i * 3 + 1] * e1 + f->x[i * 3 + 2] * e2;
             }
             __syncwarp();
             if (lane < 9) f->x[lane] = rv;
@@ -169,9 +173,10 @@ __device__ __forceinline__ void scan_const_from(const BlockFilter* f, ScanConst*
     if (tid < 9) sc->R[tid] = f->x[tid];
     else if (tid < 12) sc->p[tid - 9] = f->x[tid];
     else if (tid < 24) {
-        const int ut[6][2] = {{0, 0}, {0, 1}, {0, 2}, {1, 1}, {1, 2}, {2, 2}};
+        // entry q of the upper triangle xx xy xz yy yz zz: (i, j) computed, not read from a table indexed at run time
+        // (which would live in local memory)
         const int q = (tid - 12) % 6, o = (tid < 18) ? 0 : 3;
-        const int i = ut[q][0] + o, j = ut[q][1] + o;
+        const int i = (q < 3 ? 0 : (q < 5 ? 1 : 2)) + o, j = (q < 3 ? q : (q < 5 ? q - 2 : 2)) + o;
         const double v = 0.5 * (f->P[i * 30 + j] + f->P[j * 30 + i]);
         if (tid < 18) sc->Pth[q] = v; else sc->Ppp[q] = v;
     }
