@@ -1015,7 +1015,7 @@ static int run_range_impl(lk_handle h, uint32_t first, uint32_t count, int iters
                 launch_scan_tail(ra, first, count, s);
                 if (c1 > c0) h->acc_launches += 2;
             } else {
-                launch_residual(ra, c1 - c0, false, true, s);
+                launch_residual(ra, c1 - c0, false, s);
             }
             if (h->kernel_timing) cudaEventRecord(kev_get(h, h->nev++), s);
             if (c1 > c0) { ++h->acc_launches; ++h->acc_residual_launches; }
@@ -1190,7 +1190,7 @@ int lk_debug_residuals(lk_handle h, const lk_state* x, const double* P, const fl
     ra.dbg_z = h->dbg_z.as<double>();
     ra.dbg_R = h->dbg_R.as<double>();
     ra.dbg_key = h->dbg_key.as<int32_t>();
-    launch_residual(ra, h->total_chunks, true, false, s);
+    launch_residual(ra, h->total_chunks, true, s);
     LK_CUDA(h, cudaGetLastError());
     if (n) {
         if (ok_out) LK_CUDA(h, cudaMemcpyAsync(ok_out, h->dbg_ok.p, n, cudaMemcpyDeviceToHost, s));

@@ -10,7 +10,7 @@
 // two L2 round trips after the slowest block, moves ~10 KB per block instead of every row to every block,
 // and the sum has ONE fixed order that the multi-kernel path reproduces (block_sum_partials).
 //
-// Per-lane cache (lk_pass.cuh: cached_points_pass): a lane keeps its point, voxel keys, lookups and BOTH
+// Per-lane cache (lk_pass.cuh: points_pass): a lane keeps its point, voxel keys, lookups and BOTH
 // candidate plane records (home + the reference's one fallback neighbour, TMA-staged together) across the
 // iterations of a bucket, so iterations 2..n touch no global memory unless a key moved.
 //
@@ -61,7 +61,7 @@ struct FusedSmem {
     double clk[2];
     union {  // predict and the point passes never overlap in time
         PredictScratch pr;
-        CachedPassSmem<BLOCK> pass;
+        PassSmem<BLOCK> pass;
     } u;
 };
 
@@ -84,7 +84,7 @@ __device__ __noinline__ void fused_insert_phase2(FusedSmemIns* si, const uint32_
         warp_insert_root_scan(md, si->g, wt, __ldcg(&touched[t]), iroot, ipts, n_bucket, pend, lane);
 }
 
-static_assert(sizeof(PredictScratch) <= sizeof(((CachedPassSmem<BLOCK>*)0)->tile), "predict scratch must not reach the mbarriers");
+static_assert(sizeof(PredictScratch) <= sizeof(((PassSmem<BLOCK>*)0)->tile), "predict scratch must not reach the mbarriers");
 static_assert(sizeof(FusedSmemIns) <= 227 * 1024, "one block per SM");
 
 // KILO.cc:110-115: covariance with dt since the last UPDATE, state with dt since the last PREDICT; F is built
@@ -179,7 +179,7 @@ __global__ void __launch_bounds__(BLOCK, 1) k_scan_fused(const __grid_constant__
         if (tid == 0) si->md = a.md;
         if (tid < (int)(sizeof(Globals) / 4)) reinterpret_cast<uint32_t*>(&si->g)[tid] = reinterpret_cast<const uint32_t*>(&a.g)[tid];
     }
-    cached_pass_init<BLOCK>(&sm->u.pass);  // mbarrier init fence + block barrier
+    pass_init<BLOCK>(&sm->u.pass);  // mbarrier init fence + block barrier
     FT(1);
     uint32_t n_eff_total = 0;
     uint32_t phase = 0;
@@ -221,7 +221,8 @@ __global__ void __launch_bounds__(BLOCK, 1) k_scan_fused(const __grid_constant__
 #pragma unroll
             for (int i = 0; i < 32; ++i) acc[i] = 0.0;
             if (!a.lane_cache && lc.have == 2) lc.have = 1;
-            cached_points_pass<BLOCK, INS>(&sm->u.pass, phase, my_count, sm->sc, a.mv, a.g, acc, lc, pre);
+            points_pass<BLOCK, INS>(&sm->u.pass, phase, my_count, sm->sc, a.mv, a.g, lc, pre,
+                                    [&](uint32_t, const Row& row) { accumulate_row(row, acc); });
             FTI(14 + it_global);
             const double tot = warp_transpose_sum(acc, lane);
             sm->slice[warp * 32 + lane] = tot;

@@ -50,9 +50,9 @@ struct ResidualArgs {
 };
 constexpr uint32_t S2_FB_WARPS = 6, S2_FB_CAP = 704;
 
-// single: every chunk of the launch holds at most 256 points (one point per thread, one pass); otherwise blocks make
-// several passes over their chunk
-void launch_residual(const ResidualArgs& a, uint32_t n_chunks, bool debug, bool single, cudaStream_t s);
+// Every chunk of the launch holds at most 256 points (one point per thread, one pass), except with debug
+// (lk_debug_residuals), where a block walks its chunk in 256-point slices and writes per-point rows
+void launch_residual(const ResidualArgs& a, uint32_t n_chunks, bool debug, cudaStream_t s);
 // throughput family: pipelined residual pass (lk_stream2.cu) writing one partial row per chunk, then the per-scan
 // solve for scans [scan_first, scan_first + n_scans) (lk_residual.cu)
 void launch_residual_stream2(const ResidualArgs& a, uint32_t n_chunks, cudaStream_t s);

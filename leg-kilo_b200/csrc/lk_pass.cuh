@@ -1,13 +1,15 @@
-// lk_pass.cuh — one block-wide pass over up to NTHREADS points (one point per thread):
+// lk_pass.cuh — points_pass, one block-wide pass over up to NTHREADS points (one point per thread) through the reference's
+// residual sequence (KILO.cc:143-178). The one per-point pass of the per-scan kernel (lk_fused.cu), the single-scan residual
+// kernel and the debug rows (lk_residual.cu):
 //   1. transform, voxel key, home probe AND the speculative probe of the one neighbour voxel the
 //      reference falls back to (KILO.cc:156-178) — both 16-byte table reads are in flight together;
-//   2. every lane stages its 256-byte plane record into shared memory with one TMA bulk copy
-//      (cp.async.bulk global -> shared, completion on the warp's mbarrier) instead of 15 scattered
-//      128-bit loads per lane (32 cache lines per warp-instruction);
+//   2. every lane stages its 256-byte home and neighbour plane records into shared memory with TMA bulk
+//      copies (cp.async.bulk global -> shared, completion on the warp's mbarrier) instead of 15 scattered
+//      128-bit loads per lane and record (32 cache lines per warp-instruction);
 //   3. gates + residual row from the staged record (conflict-free 128-bit shared loads, 272-byte
 //      slot stride);
 //   4. points whose home voxel gave no residual are compacted into a block-wide list and their
-//      neighbour voxel is evaluated by the first threads of the block — a few percent of the
+//      neighbour record is evaluated by the first threads of the block — a few percent of the
 //      points fail, but almost every warp holds one, so without compaction every warp would pay
 //      the second round.
 #pragma once
@@ -17,26 +19,6 @@
 namespace lk {
 
 constexpr int TILE_STRIDE = 272;  // 256-byte record + 16: 128-bit reads of 8 consecutive lanes hit 32 banks
-
-template <int NTHREADS>
-struct PassSmem {
-    __align__(16) unsigned char tile[NTHREADS * TILE_STRIDE];
-    struct __align__(8) Fallback {
-        double pc[11];
-        int near;
-        uint32_t idx;
-    } fb[NTHREADS];
-    uint64_t bar[NTHREADS / 32];
-    uint32_t wcnt[NTHREADS / 32];  // fallback entries of each warp (its region starts at fb[warp * 32])
-};
-
-struct DebugRows {  // lk_debug_residuals outputs (nullable)
-    uint8_t* ok;
-    double* h;
-    double* z;
-    double* R;
-    int32_t* key;
-};
 
 __device__ __forceinline__ void plane_from_smem(const unsigned char* slot, PlaneRec& r) {
     const double2* q = reinterpret_cast<const double2*>(slot);
@@ -71,15 +53,6 @@ __device__ __forceinline__ void accumulate_row(const Row& row, double (&acc)[32]
     }
     acc[ACC_SUMR] += row.R;
     acc[ACC_CNT] += 1.0;
-}
-
-// Call once per block before the first pass (all threads).
-template <int NTHREADS>
-__device__ __forceinline__ void pass_init(PassSmem<NTHREADS>* ps) {
-    const int tid = threadIdx.x;
-    if ((tid & 31) == 0) mbar_init(&ps->bar[tid >> 5], 1);
-    mbar_init_fence();
-    __syncthreads();
 }
 
 // Linear probing, two slots per step: an even-aligned pair of 16-byte slots shares one 32-byte
@@ -163,21 +136,6 @@ __device__ __forceinline__ void prepare_point(float4 pt, const ScanConst& sc, co
     voxel_loc(pc, g, lx, ly, lz);
 }
 
-// Points that produced no residual at home are listed per warp in lane order (no atomics: the order, hence the
-// sums, are reproducible); entry `tid` of the warp-major concatenation of the lists is handled by thread `tid`.
-template <int NTHREADS, class PS>
-__device__ __forceinline__ void fallback_list(PS* ps, bool want, const PointCtx& pc, int near, int lane, int warp) {
-    const uint32_t m = __ballot_sync(0xffffffffu, want);
-    if (lane == 0) ps->wcnt[warp] = (uint32_t)__popc(m);
-    if (want) {
-        const uint32_t slot = (uint32_t)warp * 32u + (uint32_t)__popc(m & ((1u << lane) - 1u));
-        auto& f = ps->fb[slot];
-        f.pc[0] = pc.pbx; f.pc[1] = pc.pby; f.pc[2] = pc.pbz; f.pc[3] = pc.pix; f.pc[4] = pc.piy; f.pc[5] = pc.piz;
-        f.pc[6] = pc.pwx; f.pc[7] = pc.pwy; f.pc[8] = pc.pwz; f.pc[9] = pc.r2; f.pc[10] = pc.range2;
-        f.near = near;
-        f.idx = (uint32_t)threadIdx.x;
-    }
-}
 template <int NTHREADS, class PS>
 __device__ __forceinline__ bool fallback_pick(const PS* ps, uint32_t& fb_slot) {
     uint32_t n_fb = 0, k = threadIdx.x;
@@ -202,99 +160,14 @@ __device__ __forceinline__ bool eval_record(const MapNode* __restrict__ nodes, c
     return false;
 }
 
-// One pass, every point looked up afresh (multi-kernel path). `phase` is the warp's mbarrier parity (start at 0,
-// carried between passes). base_idx = absolute index of pts[0] (debug output addressing).
-template <int NTHREADS, bool DEBUG>
-__device__ __forceinline__ void block_points_pass(PassSmem<NTHREADS>* ps, uint32_t& phase, const float4* __restrict__ pts,
-                                                  uint32_t count, size_t base_idx, const ScanConst& sc, const MapView& mv,
-                                                  const Globals& g, double (&acc)[32], const DebugRows& dbg) {
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const bool active = (uint32_t)tid < count;
-    PointCtx pc;
-    int root = -1, near = -1;
-    int key[3] = {0, 0, 0};
-    if (active) {
-        float lx, ly, lz;
-        prepare_point(__ldg(pts + tid), sc, g, pc, lx, ly, lz);
-        const int kx = (int)lx, ky = (int)ly, kz = (int)lz;
-        key[0] = kx; key[1] = ky; key[2] = kz;
-        int nx, ny, nz;
-        neighbour_key(g, lx, ly, lz, kx, ky, kz, nx, ny, nz);
-        const bool differs = (nx != kx) || (ny != ky) || (nz != kz);
-        // both home pairs are read before either is inspected
-        const uint32_t ih = hash_key(kx, ky, kz) & mv.hash_mask, in = hash_key(nx, ny, nz) & mv.hash_mask;
-        const SlotPair sh = load_pair(mv.slots, ih);
-        const SlotPair sn = load_pair(mv.slots, in);
-        root = resolve_pair(mv.slots, mv.hash_mask, ih, sh, kx, ky, kz);
-        // the reference only looks at the neighbour when the home voxel exists
-        near = (root >= 0 && differs) ? resolve_pair(mv.slots, mv.hash_mask, in, sn, nx, ny, nz) : -1;
-    }
-    // ---- stage the home records: one bulk copy per lane -------------------------------------------
-    unsigned char* my_slot = ps->tile + (size_t)tid * TILE_STRIDE;
-    const bool gather = root >= 0;
-    const uint32_t valid = __ballot_sync(0xffffffffu, gather);
-    if (valid) {
-        if (lane == 0) mbar_expect_tx(&ps->bar[warp], 256u * (uint32_t)__popc(valid));
-        __syncwarp();
-        if (gather) bulk_g2s(my_slot, mv.nodes + root, 256u, &ps->bar[warp]);
-        mbar_wait(&ps->bar[warp], phase);
-        phase ^= 1u;
-    }
-    // ---- gates + row -----------------------------------------------------------------------------
-    Row row;
-    bool ok = false;
-    if (root >= 0) {
-        PlaneRec r;
-        plane_from_smem(my_slot, r);
-        ok = eval_record(mv.nodes, r, pc, sc, g, row);
-    }
-    fallback_list<NTHREADS>(ps, root >= 0 && !ok && near >= 0, pc, near, lane, warp);
-    if (DEBUG) {
-        if (active) {
-            const size_t gi = base_idx + tid;
-            dbg.ok[gi] = ok ? 1 : 0;
-            for (int k = 0; k < 3; ++k) dbg.key[gi * 3 + k] = key[k];
-            for (int k = 0; k < 6; ++k) dbg.h[gi * 6 + k] = ok ? row.h[k] : 0.0;
-            dbg.z[gi] = ok ? row.z : 0.0;
-            dbg.R[gi] = ok ? row.R : 0.0;
-        }
-    }
-    __syncthreads();
-    // ---- fallback round: the neighbour voxel of the points that failed at home ------------------------
-    uint32_t fb_slot = 0;
-    Row row2;
-    bool ok2 = false;
-    if (fallback_pick<NTHREADS>(ps, fb_slot)) {
-        const typename PassSmem<NTHREADS>::Fallback& f = ps->fb[fb_slot];
-        PointCtx fc;
-        fc.pbx = f.pc[0]; fc.pby = f.pc[1]; fc.pbz = f.pc[2]; fc.pix = f.pc[3]; fc.piy = f.pc[4]; fc.piz = f.pc[5];
-        fc.pwx = f.pc[6]; fc.pwy = f.pc[7]; fc.pwz = f.pc[8]; fc.r2 = f.pc[9]; fc.range2 = f.pc[10];
-        PlaneRec r;
-        load_plane(mv.nodes + f.near, r);
-        ok2 = eval_record(mv.nodes, r, fc, sc, g, row2);
-        if (ok2 && DEBUG) {
-            const size_t gi = base_idx + f.idx;
-            dbg.ok[gi] = 1;
-            for (int k = 0; k < 6; ++k) dbg.h[gi * 6 + k] = row2.h[k];
-            dbg.z[gi] = row2.z;
-            dbg.R[gi] = row2.R;
-        }
-    }
-    if (!DEBUG) {  // rows are folded in only now, so no accumulator is live across the evaluations
-        if (ok) accumulate_row(row, acc);
-        if (ok2) accumulate_row(row2, acc);
-    }
-    __syncthreads();
-}
-
 // =================================================================================================
-// Cached pass of the fused per-scan kernel (one chunk per block, so a lane sees the same point in every iteration
-// of a bucket). A lane keeps everything that does not depend on the state, plus the last voxel key with its lookup
-// results; BOTH candidate records — the home voxel's and the one neighbour voxel's the reference falls back to
+// The block-wide pass. In the fused per-scan kernel a block keeps one chunk, so a lane sees the same point in every
+// iteration of a bucket: the lane keeps everything that does not depend on the state, plus the last voxel key with its
+// lookup results; BOTH candidate records — the home voxel's and the one neighbour voxel's the reference falls back to
 // (KILO.cc:156-178) — are staged into shared memory by TMA bulk copies issued together, and stay there: when the key
 // is unchanged in a later iteration (the map is static within a bucket) the probes AND the gathers are skipped, and
 // the fallback round reads its record from shared memory instead of paying another dependent global round trip.
-// Arithmetic and accumulation order are those of block_points_pass (bitwise-equal sums).
+// A kernel that sees each point once starts every pass with a fresh LaneCache (have = 0).
 // =================================================================================================
 struct LaneCache {
     double pbx, pby, pbz, pix, piy, piz, r2, range2;
@@ -303,7 +176,7 @@ struct LaneCache {
 };
 
 template <int NTHREADS>
-struct CachedPassSmem {
+struct PassSmem {
     __align__(16) unsigned char tile[2][NTHREADS * TILE_STRIDE];  // [0] home records, [1] neighbour records
     // Every lane's point context of the current pass. The evaluations read it from here and the descent receives its
     // address, so it never lives in the stack frame (which the L1 left beside this much shared memory cannot hold: every
@@ -318,17 +191,19 @@ struct CachedPassSmem {
 };
 
 template <int NTHREADS>
-__device__ __forceinline__ void cached_pass_init(CachedPassSmem<NTHREADS>* ps) {
+__device__ __forceinline__ void pass_init(PassSmem<NTHREADS>* ps) {
     const int tid = threadIdx.x;
     if ((tid & 31) == 0) mbar_init(&ps->bar[tid >> 5], 1);
     mbar_init_fence();
     __syncthreads();
 }
 
-template <int NTHREADS, bool COH = false>
-__device__ __forceinline__ void cached_points_pass(CachedPassSmem<NTHREADS>* ps, uint32_t& phase, uint32_t count,
-                                                   const ScanConst& sc, const MapView& mv, const Globals& g,
-                                                   double (&acc)[32], LaneCache& lc, float4 pre) {
+// `phase` is the warp's mbarrier parity (start at 0, carried between passes). Every row goes to sink(idx, row), `idx` being
+// the thread that holds the point: a thread passes its own home row, then the fallback row it evaluated for another
+// thread. Both calls follow both evaluations, so nothing the sink keeps (the accumulators) is live across an evaluation.
+template <int NTHREADS, bool COH = false, class Sink>
+__device__ __forceinline__ void points_pass(PassSmem<NTHREADS>* ps, uint32_t& phase, uint32_t count, const ScanConst& sc,
+                                            const MapView& mv, const Globals& g, LaneCache& lc, float4 pre, Sink sink) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const bool active = (uint32_t)tid < count;
     PointCtx& pc = ps->pt[tid];
@@ -402,7 +277,8 @@ __device__ __forceinline__ void cached_points_pass(CachedPassSmem<NTHREADS>* ps,
         plane_from_smem(home_slot, r);
         ok = eval_record<COH>(mv.nodes, r, pc, sc, g, row);
     }
-    {  // the failing points, listed per warp in lane order as fallback_list does; their contexts stay in pt
+    {  // the failing points, listed per warp in lane order (no atomics: the order, hence the sums, are reproducible); entry
+       // `tid` of the warp-major concatenation of the lists is handled by thread `tid`; their contexts stay in pt
         const bool want = root >= 0 && !ok && near >= 0;
         const uint32_t m = __ballot_sync(0xffffffffu, want);
         if (lane == 0) ps->wcnt[warp] = (uint32_t)__popc(m);
@@ -414,19 +290,18 @@ __device__ __forceinline__ void cached_points_pass(CachedPassSmem<NTHREADS>* ps,
     }
     __syncthreads();
     // ---- fallback round: the neighbour voxel of the points that failed at home, record already staged -------
-    uint32_t fb_slot = 0;
+    uint32_t fb_slot = 0, idx = 0;
     Row row2;
     bool ok2 = false;
     if (fallback_pick<NTHREADS>(ps, fb_slot)) {
-        const uint32_t idx = ps->fb[fb_slot].idx;
+        idx = ps->fb[fb_slot].idx;
         PlaneRec r;
         plane_from_smem(ps->tile[1] + (size_t)idx * TILE_STRIDE, r);
         ok2 = eval_record<COH>(mv.nodes, r, ps->pt[idx], sc, g, row2);
     }
-    if (ok) accumulate_row(row, acc);
-    if (ok2) accumulate_row(row2, acc);
+    if (ok) sink((uint32_t)tid, row);
+    if (ok2) sink(idx, row2);
     __syncthreads();  // the fallback list is rewritten by the next pass
 }
-
 
 }  // namespace lk

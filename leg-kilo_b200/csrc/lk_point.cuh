@@ -1,6 +1,7 @@
-// lk_point.cuh — one LiDAR point through rows a3-a7 of SURVEY.md §8a, and the warp-level
-// reduction / 6x6 solve primitives. Shared by the batched multi-kernel path (lk_residual.cu) and
-// the fused per-scan persistent kernel (lk_fused.cu).
+// lk_point.cuh — the per-point evaluations of rows a3-a7 of SURVEY.md §8a (plane record, gates + row, octree descent)
+// that the block-wide pass (lk_pass.cuh) is built from; point_row, one point through the whole sequence straight from
+// global memory for the throughput family's fallback kernel (lk_stream2.cu); and the warp-level reduction / 6x6 solve
+// primitives.
 //
 // Follows: a3 KILO.cc:127-140 + voxel_map.cc:22-40, a4 KILO.cc:143-149, a5 voxel_map.cc:363-427,
 // a6 KILO.cc:156-178, a7 KILO.cc:187-210. Algebra is restructured (never the results' meaning):

@@ -1,6 +1,7 @@
-// lk_residual.cu — the hot kernel: per point transform -> voxel key -> hash probe -> plane gates ->
-// residual / Jacobian row -> block-reduced H^T R^-1 H, H^T R^-1 z; the last block of every scan
-// does the 6x6 information-form Kalman solve and the state / covariance update.
+// lk_residual.cu — one scan on the multi-kernel path: the per-point pass of lk_pass.cuh (transform -> voxel key ->
+// hash probes -> staged records -> plane gates -> residual / Jacobian row, the one neighbour voxel on failure) ->
+// block-reduced H^T R^-1 H, H^T R^-1 z; the last block of every scan does the 6x6 information-form Kalman solve and the
+// state / covariance update. The same pass writes the per-point rows of lk_debug_residuals.
 //
 // Follows, row by row (SURVEY.md §8a): a3 KILO.cc:127-140 + voxel_map.cc:22-40, a4 KILO.cc:143-149,
 // a5 voxel_map.cc:363-427, a6 KILO.cc:156-178, a7 KILO.cc:187-210, a8 eskf.cc:91-113,
@@ -62,15 +63,16 @@ __device__ void scan_solve(const ResidualArgs& a, uint32_t scan, TailSmem* ts) {
     }
 }
 
-union ResidualSmem {  // the tail runs after the passes: same storage
+union ResidualSmem {  // the tail runs after the pass: same storage
     PassSmem<BLOCK> pass;
     TailSmem tail;
 };
 
-// SINGLE: every chunk has at most BLOCK points (one pass, latency mode) so no accumulator is live
-// while a point is being evaluated; otherwise the block makes several passes over its chunk.
-template <bool DEBUG, bool SINGLE>
-__global__ void __launch_bounds__(BLOCK, (DEBUG || SINGLE) ? 1 : 2) k_residual(const __grid_constant__ ResidualArgs a) {
+// One pass over the block's chunk (at most BLOCK points on this path), its rows summed into the chunk's partial row; the last
+// block of a scan solves. DEBUG (lk_debug_residuals): the chunk may be longer, so the block walks it in BLOCK-point slices and
+// writes every point's row and voxel key instead of summing.
+template <bool DEBUG>
+__global__ void __launch_bounds__(BLOCK, 1) k_residual(const __grid_constant__ ResidualArgs a) {
     extern __shared__ __align__(16) unsigned char s_raw[];
     __shared__ ScanConst s_sc;
     __shared__ uint32_t s_last;
@@ -85,20 +87,45 @@ __global__ void __launch_bounds__(BLOCK, (DEBUG || SINGLE) ? 1 : 2) k_residual(c
     LK_TRACE(1);
     MapView mv;
     mv.slots = a.slots; mv.hash_mask = a.hash_mask; mv.nodes = a.nodes;
-    DebugRows dbg;
-    dbg.ok = a.dbg_ok; dbg.h = a.dbg_h; dbg.z = a.dbg_z; dbg.R = a.dbg_R; dbg.key = a.dbg_key;
-
     double acc[32];
 #pragma unroll
     for (int i = 0; i < 32; ++i) acc[i] = 0.0;
     uint32_t phase = 0;
-    for (uint32_t off = 0; off < cd.count; off += BLOCK) {
-        const uint32_t n = min((uint32_t)BLOCK, cd.count - off);
-        block_points_pass<BLOCK, DEBUG>(&rs->pass, phase, a.pts + cd.start + off, n, (size_t)cd.start + off, s_sc, mv, a.g,
-                                        acc, dbg);
-        if (SINGLE) break;
+    if (DEBUG) {
+        for (uint32_t off = 0; off < cd.count; off += BLOCK) {
+            const uint32_t n = min((uint32_t)BLOCK, cd.count - off);
+            const size_t base = (size_t)cd.start + off;
+            LaneCache lc;
+            lc.have = 0;
+            float4 pre = make_float4(0.f, 0.f, 0.f, 0.f);
+            if ((uint32_t)tid < n) {  // no row yet; the fallback row of this point may come from another thread, after a barrier
+                pre = __ldg(a.pts + base + tid);
+                a.dbg_ok[base + tid] = 0;
+                for (int k = 0; k < 6; ++k) a.dbg_h[(base + tid) * 6 + k] = 0.0;
+                a.dbg_z[base + tid] = 0.0;
+                a.dbg_R[base + tid] = 0.0;
+            }
+            points_pass<BLOCK>(&rs->pass, phase, n, s_sc, mv, a.g, lc, pre, [&](uint32_t idx, const Row& row) {
+                const size_t gi = base + idx;
+                a.dbg_ok[gi] = 1;
+                for (int k = 0; k < 6; ++k) a.dbg_h[gi * 6 + k] = row.h[k];
+                a.dbg_z[gi] = row.z;
+                a.dbg_R[gi] = row.R;
+            });
+            if ((uint32_t)tid < n) {
+                a.dbg_key[(base + tid) * 3 + 0] = lc.kx;
+                a.dbg_key[(base + tid) * 3 + 1] = lc.ky;
+                a.dbg_key[(base + tid) * 3 + 2] = lc.kz;
+            }
+        }
+        return;
     }
-    if (DEBUG) return;
+    const uint32_t n = min((uint32_t)BLOCK, cd.count);
+    LaneCache lc;
+    lc.have = 0;
+    float4 pre = make_float4(0.f, 0.f, 0.f, 0.f);
+    if ((uint32_t)tid < n) pre = __ldg(a.pts + cd.start + tid);
+    points_pass<BLOCK>(&rs->pass, phase, n, s_sc, mv, a.g, lc, pre, [&](uint32_t, const Row& row) { accumulate_row(row, acc); });
     LK_TRACE(2);
 
     // block reduction: transposing shuffle tree in the warp, one row per warp in smem, fixed-order sum
@@ -150,22 +177,18 @@ void launch_scan_tail(const ResidualArgs& a, uint32_t scan_first, uint32_t n_sca
     k_scan_tail<<<n_scans, BLOCK, sizeof(TailSmem), s>>>(a, scan_first);
 }
 
-void launch_residual(const ResidualArgs& a, uint32_t n_chunks, bool debug, bool single, cudaStream_t s) {
+void launch_residual(const ResidualArgs& a, uint32_t n_chunks, bool debug, cudaStream_t s) {
     if (n_chunks == 0) return;
     static PerDeviceOnce once;
     const size_t smem = sizeof(ResidualSmem);
     if (once.first()) {
-        cudaFuncSetAttribute(k_residual<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        cudaFuncSetAttribute(k_residual<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        cudaFuncSetAttribute(k_residual<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        cudaFuncSetAttribute(k_residual<false, false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+        cudaFuncSetAttribute(k_residual<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        cudaFuncSetAttribute(k_residual<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     }
     if (debug)
-        k_residual<true, false><<<n_chunks, BLOCK, smem, s>>>(a);
-    else if (single)
-        k_residual<false, true><<<n_chunks, BLOCK, smem, s>>>(a);
+        k_residual<true><<<n_chunks, BLOCK, smem, s>>>(a);
     else
-        k_residual<false, false><<<n_chunks, BLOCK, smem, s>>>(a);
+        k_residual<false><<<n_chunks, BLOCK, smem, s>>>(a);
 }
 
 // ---- re-projection with the updated state (KILO.cc:216-224) ---------------------------------

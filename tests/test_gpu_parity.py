@@ -39,8 +39,8 @@ def test_config1_planar_literal_pin():
     assert out["clk"]["last_update_time"][0] == clko["last_update_time"][0]
 
 
-def test_debug_rows_match_oracle():
-    cfg, blob, pts = scenes.planar_scene(n=1500, seed_stream=7)
+def _check_debug_rows(n):
+    cfg, blob, pts = scenes.planar_scene(n=n, seed_stream=7)
     x0 = abi.default_states(1); P0 = abi.init_cov(1)
     ro, _, _, _ = _oracle_bucket(cfg, blob, pts, x0, P0)
     eng = Engine(cfg)
@@ -52,6 +52,15 @@ def test_debug_rows_match_oracle():
     # eigenvector sign is free: compare sign-invariant products
     np.testing.assert_allclose(d["h"][m] * d["z"][m, None], ro["h"][m] * ro["z"][m, None], rtol=1e-9, atol=1e-12)
     np.testing.assert_allclose(d["R"][m], ro["R"][m], rtol=1e-9)
+
+
+def test_debug_rows_match_oracle():
+    _check_debug_rows(1500)
+
+
+def test_debug_rows_match_oracle_sliced_chunks():
+    """One bucket above 132 x 256 points gets 3 840-point chunks, which the debug kernel walks in 256-point slices."""
+    _check_debug_rows(40000)
 
 
 @pytest.mark.parametrize("iters", [1, 3])
