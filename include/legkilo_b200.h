@@ -228,8 +228,18 @@ int lk_map_stats(lk_handle h, uint64_t out[4]);
  * runs): when `position` is at least sliding_thresh away from the position of the last slide (initially the origin,
  * voxel_map.h:201), every root voxel whose key lies outside [k - half_map_size, k + half_map_size] on some axis,
  * k = floor(position / voxel_size) (eigen_types.hpp:89-95), is removed from the map. *slid = 1 when a slide happened,
- * *removed = root voxels dropped. The root table is rebuilt; pool storage of the dropped octrees is not recycled. */
+ * *removed = root voxels dropped. The root table is rebuilt, and the dropped octrees' nodes and standard point tiles
+ * go to the map's free lists, from which the next scan that updates the map allocates before it grows the pools. */
 int lk_map_slide(lk_handle h, const double position[3], int32_t* slid, uint64_t* removed);
+/* Device memory of the map, for long runs that must check it has stopped growing:
+ * out[0] = node slots handed out by the bump allocator, out[1] = nodes on the free lists,
+ * out[2] = point slots handed out by the bump allocator, out[3] = point slots on the free lists,
+ * out[4] = device bytes of the map pools as allocated, out[5] = pool reallocations since the map was created.
+ * Storage is recycled where the map stops using it: the point tile of a leaf that freezes at max_points_num, the tile
+ * of a node whose points were cut into octants, and whole octrees dropped by lk_map_slide. An entry freed by one
+ * launch is reused from the next launch that updates the map on. out[0] - out[1] nodes and out[2] - out[3] slots are
+ * held; only tiles of the standard max_points_num + 2 (even) slots are recycled. */
+int lk_map_memory(lk_handle h, uint64_t out[6]);
 
 /* ---- the hot path ---------------------------------------------------------------------- */
 

@@ -193,6 +193,7 @@ void fill_globals(lk_context* c, const double* extR, const double* extT) {
     g.max_layer = c->mc.max_layer;
     g.max_points_num = c->mc.max_points_num;
     for (int i = 0; i < 5; ++i) g.layer_init_num[i] = c->mc.layer_init_num[i];
+    c->map.tile_slots = (uint32_t)((std::max(g.max_points_num, 0) + 2 + 1) & ~1);  // lk_octree.cuh: std_tile
 }
 
 // the trace buffer ((1 << 16) * 8 doubles' worth of %globaltimer stamps): TRACE_AREAS areas of TRACE_AREA stamps, one per
@@ -453,6 +454,23 @@ int lk_map_stats(lk_handle h, uint64_t out[4]) {
     out[1] = h->map.n_nodes;
     out[2] = live;
     out[3] = planes;
+    return LK_OK;
+}
+
+int lk_map_memory(lk_handle h, uint64_t out[6]) {
+    if (!h || !out) return LK_ERR_INVALID_ARG;
+    cudaSetDevice(h->device);
+    h->prev_fused = false;
+    std::string err;
+    MapDevHost& m = h->map;
+    const int rc = m.ready() ? m.sync_counters(h->stream, err) : LK_OK;
+    if (rc) return fail(h, rc, err);
+    out[0] = m.n_nodes;
+    out[1] = 8 * m.free_entries(FREE_GROUPS) + m.free_entries(FREE_SINGLES);
+    out[2] = m.n_points;
+    out[3] = (uint64_t)m.tile_slots * m.free_entries(FREE_TILES);
+    out[4] = m.pool_bytes();
+    out[5] = m.reallocs;
     return LK_OK;
 }
 
@@ -809,7 +827,7 @@ static int run_range_impl(lk_handle h, uint32_t first, uint32_t count, int iters
             const uint64_t per_pt_slots = tile * (1 + (uint64_t)std::max(g.max_layer, 0) * (uint64_t)std::min(8, thr + 1)) + 2;
             rc = h->map.ensure_headroom(n + 16, per_pt_nodes * n + 64, per_pt_slots * n + 64, s, err);
         }
-        if (!rc) rc = h->map.push_counters(s, err);
+        if (!rc) rc = h->map.push_counters(s, err);  // also makes what earlier launches freed available to this scan
         if (rc) return fail(h, rc, err);
         for (uint32_t k = 0; k < h->n_steps; ++k) {
             const StepInit& in = h->h_inits[(size_t)k * batch + first];

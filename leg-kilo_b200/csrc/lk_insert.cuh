@@ -17,7 +17,8 @@ __device__ __forceinline__ int hash_find_or_create(MapDev& md, const Globals& g,
             int old = atomicCAS(nodep, -1, -2);
             if (old == -1) {
                 md.slots[i].kx = kx; md.slots[i].ky = ky; md.slots[i].kz = kz;
-                uint32_t nd = atomicAdd(md.n_nodes, 1u);
+                uint32_t nd;
+                if (!free_pop(md, FREE_SINGLES, nd)) nd = atomicAdd(md.n_nodes, 1u);  // a slid-out root's node first
                 if (nd >= md.node_cap) {
                     atomicOr(md.overflow, 1u);
                     __threadfence();

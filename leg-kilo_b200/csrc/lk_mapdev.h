@@ -21,20 +21,38 @@ class MapDevHost {
     void release();
     MapDev dev() const;
     bool ready() const { return hash_cap != 0; }
-    // pull the device allocator counters into the host mirrors
+    // pull the device allocator counters (free lists included) into the host mirrors
     int sync_counters(cudaStream_t s, std::string& err);
+    // push the host mirrors; the free-list entries pushed since the last push become available (needs a sync_counters
+    // after the last launch that freed anything)
     int push_counters(cudaStream_t s, std::string& err);
+    // entries on free list l (FREE_TILES / FREE_GROUPS / FREE_SINGLES), available or pending, as of the last sync
+    uint64_t free_entries(int l) const;
+    uint64_t pool_bytes() const;
 
     HashSlot* slots = nullptr;
     MapNode* nodes = nullptr;
     MapAux* aux = nullptr;
     HotRec* hot = nullptr;  // hot image of every node's plane (what the throughput kernel gathers)
     DevPoint* points = nullptr;
-    uint32_t* counters = nullptr;  // [0] n_nodes [1] n_roots [2] overflow [4..5] n_points (u64)
+    // [0] n_nodes [1] n_roots [2] overflow [4..5] n_points (u64) [8] scratch [10..13] map_count_planes
+    // [16 + 3 l .. 18 + 3 l] avail | base | top of free list l (MapDev::free_ctr)
+    uint32_t* counters = nullptr;
     uint64_t hash_cap = 0, node_cap = 0, point_cap = 0;
     uint32_t n_roots = 0, n_nodes = 0;
     uint64_t n_points = 0;  // bump pointer (slots handed out), not the number of live points
     uint64_t reserve_roots = 0, reserve_nodes = 0, reserve_points = 0;
+    uint32_t tile_slots = 52;  // the standard point tile, even_up(max_points_num + 2) (set with the map config)
+    // free lists: twice as many entries as the pool holds tiles / groups / nodes, so a launch that pops and then frees
+    // every object again still finds room for the pending entries
+    uint32_t* free_items[3] = {nullptr, nullptr, nullptr};
+    uint64_t free_cap[3] = {0, 0, 0};
+    int32_t free_avail[3] = {0, 0, 0};
+    uint32_t free_base[3] = {0, 0, 0}, free_top[3] = {0, 0, 0};
+    uint64_t reallocs = 0;  // pool growths since the map was created
+
+   private:
+    int size_free_lists(bool keep, cudaStream_t s, std::string& err);
 };
 
 // lk_mapbuild.cu

@@ -1,5 +1,6 @@
 // lk_mapio.cu — device map storage management and the blob import / export
 // (lk_map_upload / lk_map_download of include/legkilo_b200.h).
+#include <algorithm>
 #include <cstring>
 #include <vector>
 
@@ -60,6 +61,36 @@ __global__ void k_count_planes(const MapNode* nodes, const MapAux* aux, uint32_t
     if (aux[i].pts_count > 0) atomicAdd(out + 1, (unsigned long long)aux[i].pts_count);
 }
 
+// The storage of the octrees under dropped roots goes back to the free lists: one thread per root walks the subtree
+// through child_base and the child mask, pushes the standard tiles still held, every 8-node child group and the root
+// node, and resets each node to the empty state (hot record included). The nodes are unreachable: the table no longer
+// holds their keys.
+__global__ void k_free_subtrees(MapDev md, const lk_map_root* gone, uint32_t n, int tile) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint32_t root = (uint32_t)gone[i].node;
+    free_push(md, FREE_SINGLES, root);
+    uint32_t stack[8 * 6];  // depth-first: at most 7 pending siblings per level below the root (layer <= 4)
+    int sp = 0;
+    stack[sp++] = root;
+    while (sp > 0) {
+        const uint32_t nd = stack[--sp];
+        const uint32_t flags = md.nodes[nd].flags;
+        const int cb = md.nodes[nd].child_base;
+        const MapAux& a = md.aux[nd];
+        if (a.pts_cap == tile && a.pts_base != NO_TILE) free_push(md, FREE_TILES, a.pts_base);
+        if (cb >= 0) {
+            free_push(md, FREE_GROUPS, (uint32_t)cb);
+            const uint32_t mask = (flags >> LK_NODE_CHILDMASK_SHIFT) & 0xffu;
+            for (int c = 0; c < 8; ++c) {
+                if (!((mask >> c) & 1u)) node_reset(md, (uint32_t)cb + c, 0, -1);
+                else if (sp < 8 * 6) stack[sp++] = (uint32_t)cb + c;
+            }
+        }
+        node_reset(md, nd, 0, -1);
+    }
+}
+
 uint64_t next_pow2(uint64_t v) {
     uint64_t p = 1;
     while (p < v) p <<= 1;
@@ -78,14 +109,53 @@ uint64_t next_pow2(uint64_t v) {
 
 }  // namespace
 
+constexpr size_t COUNTER_BYTES = 128;
+constexpr int FREE_CTR = 16;  // first counter word of the free lists
+
 void MapDevHost::release() {
-    void* ptrs[] = {slots, nodes, aux, hot, points, counters};
+    void* ptrs[] = {slots, nodes, aux, hot, points, counters, free_items[0], free_items[1], free_items[2]};
     for (void* p : ptrs)
         if (p) cudaFree(p);
     slots = nullptr; nodes = nullptr; aux = nullptr; hot = nullptr; points = nullptr; counters = nullptr;
     hash_cap = node_cap = point_cap = 0;
     n_roots = n_nodes = 0;
     n_points = 0;
+    for (int l = 0; l < 3; ++l) {
+        free_items[l] = nullptr;
+        free_cap[l] = 0;
+        free_avail[l] = 0; free_base[l] = free_top[l] = 0;
+    }
+    reallocs = 0;
+}
+
+// Grow the free-list arrays to twice the entries the pools can hold. keep: copy the entries of the old arrays (the
+// mirrors are those of a sync after the last launch); else the lists start empty.
+int MapDevHost::size_free_lists(bool keep, cudaStream_t s, std::string& err) {
+    const uint64_t want[3] = {2 * (point_cap / std::max<uint32_t>(tile_slots, 2)) + 2, 2 * (node_cap / 8) + 2, 2 * node_cap + 2};
+    for (int l = 0; l < 3; ++l) {
+        if (!keep) { free_avail[l] = 0; free_base[l] = free_top[l] = 0; }
+        if (want[l] <= free_cap[l]) continue;
+        uint32_t* p = nullptr;
+        MI_CUDA(cudaMalloc((void**)&p, want[l] * sizeof(uint32_t)));
+        const uint64_t used = keep ? std::min<uint64_t>(free_top[l], free_cap[l]) : 0;
+        if (used) MI_CUDA(cudaMemcpyAsync(p, free_items[l], used * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
+        MI_CUDA(cudaStreamSynchronize(s));
+        if (free_items[l]) cudaFree(free_items[l]);
+        free_items[l] = p;
+        free_cap[l] = want[l];
+    }
+    return LK_OK;
+}
+
+uint64_t MapDevHost::free_entries(int l) const {
+    return (uint64_t)std::max(free_avail[l], 0) + (std::min<uint64_t>(free_top[l], free_cap[l]) - free_base[l]);
+}
+
+uint64_t MapDevHost::pool_bytes() const {
+    uint64_t b = hash_cap * sizeof(HashSlot) + node_cap * (sizeof(MapNode) + sizeof(MapAux) + sizeof(HotRec)) +
+                 point_cap * sizeof(DevPoint) + (counters ? COUNTER_BYTES : 0);
+    for (int l = 0; l < 3; ++l) b += free_cap[l] * sizeof(uint32_t);
+    return b;
 }
 
 MapDev MapDevHost::dev() const {
@@ -102,6 +172,11 @@ MapDev MapDevHost::dev() const {
     d.n_roots = counters + 1;
     d.overflow = counters + 2;
     d.n_points = reinterpret_cast<unsigned long long*>(counters + 4);
+    for (int l = 0; l < 3; ++l) {
+        d.free_items[l] = free_items[l];
+        d.free_cap[l] = (uint32_t)std::min<uint64_t>(free_cap[l], 0xffffffffu);
+    }
+    d.free_ctr = counters ? counters + FREE_CTR : nullptr;
     return d;
 }
 
@@ -112,7 +187,7 @@ int MapDevHost::allocate(uint64_t roots, uint64_t nnodes, uint64_t npoints, cuda
     uint64_t want_points = std::max<uint64_t>(npoints + reserve_points, 64);
     if (want_nodes >= (1ull << 31)) { err = "node pool too large"; return LK_ERR_CAPACITY; }
     if (want_points >= (1ull << 32)) { err = "point pool too large"; return LK_ERR_CAPACITY; }
-    if (!counters) MI_CUDA(cudaMalloc((void**)&counters, 64));
+    if (!counters) MI_CUDA(cudaMalloc((void**)&counters, COUNTER_BYTES));
     if (want_hash != hash_cap) {
         if (slots) cudaFree(slots);
         slots = nullptr; hash_cap = 0;
@@ -135,11 +210,14 @@ int MapDevHost::allocate(uint64_t roots, uint64_t nnodes, uint64_t npoints, cuda
         MI_CUDA(cudaMalloc((void**)&points, want_points * sizeof(DevPoint)));
         point_cap = want_points;
     }
+    int rc = size_free_lists(false, s, err);  // a new map starts with empty free lists
+    if (rc) return rc;
     k_hash_clear<<<(unsigned)((hash_cap + 255) / 256), 256, 0, s>>>(slots, hash_cap);
-    MI_CUDA(cudaMemsetAsync(counters, 0, 64, s));
+    MI_CUDA(cudaMemsetAsync(counters, 0, COUNTER_BYTES, s));
     MI_CUDA(cudaGetLastError());
     n_roots = n_nodes = 0;
     n_points = 0;
+    reallocs = 0;
     return LK_OK;
 }
 
@@ -162,6 +240,7 @@ int MapDevHost::ensure_headroom(uint64_t extra_roots, uint64_t extra_nodes, uint
         MI_CUDA(cudaStreamSynchronize(s));
         cudaFree(nodes); cudaFree(aux); cudaFree(hot);
         nodes = nn; aux = na; hot = nh; node_cap = want;
+        ++reallocs;
     }
     if (n_points + extra_points > point_cap) {
         uint64_t want = std::max<uint64_t>(n_points + extra_points, point_cap + point_cap / 2);
@@ -172,7 +251,10 @@ int MapDevHost::ensure_headroom(uint64_t extra_roots, uint64_t extra_nodes, uint
         MI_CUDA(cudaStreamSynchronize(s));
         cudaFree(points);
         points = np; point_cap = want;
+        ++reallocs;
     }
+    int rc = size_free_lists(true, s, err);
+    if (rc) return rc;
     if (4 * (n_roots + extra_roots) > hash_cap) {
         // rehash: dump roots, rebuild a bigger table
         uint64_t want = next_pow2(4 * (n_roots + extra_roots) + 4 * reserve_roots);
@@ -189,27 +271,49 @@ int MapDevHost::ensure_headroom(uint64_t extra_roots, uint64_t extra_nodes, uint
         MI_CUDA(cudaStreamSynchronize(s));
         cudaFree(slots); cudaFree(tmp);
         slots = ns; hash_cap = want;
+        ++reallocs;
     }
     return LK_OK;
 }
 
 int MapDevHost::sync_counters(cudaStream_t s, std::string& err) {
-    uint32_t h[6] = {0, 0, 0, 0, 0, 0};
-    MI_CUDA(cudaMemcpyAsync(h, counters, 24, cudaMemcpyDeviceToHost, s));
+    uint32_t h[FREE_CTR + 9] = {};
+    MI_CUDA(cudaMemcpyAsync(h, counters, sizeof(h), cudaMemcpyDeviceToHost, s));
     MI_CUDA(cudaStreamSynchronize(s));
     n_nodes = h[0];
     n_roots = h[1];
     unsigned long long np;
     std::memcpy(&np, &h[4], 8);
     n_points = np;
+    for (int l = 0; l < 3; ++l) {
+        free_avail[l] = (int32_t)h[FREE_CTR + 3 * l];
+        free_base[l] = h[FREE_CTR + 3 * l + 1];
+        free_top[l] = h[FREE_CTR + 3 * l + 2];
+    }
     return LK_OK;
 }
 
 int MapDevHost::push_counters(cudaStream_t s, std::string& err) {
-    uint32_t h[6] = {n_nodes, n_roots, 0, 0, 0, 0};
+    // Promote: the entries pushed since the last push, [base, top), join the available ones. Pops left a hole
+    // [avail, base); the last min(hole, pending) entries move into it (disjoint ranges, order is irrelevant).
+    for (int l = 0; l < 3; ++l) {
+        const uint32_t a = (uint32_t)std::max(free_avail[l], 0);
+        const uint32_t b = free_base[l];
+        const uint32_t t = (uint32_t)std::min<uint64_t>(free_top[l], free_cap[l]);
+        const uint32_t pend = t - b, k = std::min(b - a, pend);
+        if (k) MI_CUDA(cudaMemcpyAsync(free_items[l] + a, free_items[l] + (t - k), (size_t)k * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
+        free_avail[l] = (int32_t)(a + pend);
+        free_base[l] = free_top[l] = a + pend;
+    }
+    uint32_t h[FREE_CTR + 9] = {n_nodes, n_roots};
     unsigned long long np = n_points;
     std::memcpy(&h[4], &np, 8);
-    MI_CUDA(cudaMemcpyAsync(counters, h, 24, cudaMemcpyHostToDevice, s));
+    for (int l = 0; l < 3; ++l) {
+        h[FREE_CTR + 3 * l] = (uint32_t)free_avail[l];
+        h[FREE_CTR + 3 * l + 1] = free_base[l];
+        h[FREE_CTR + 3 * l + 2] = free_top[l];
+    }
+    MI_CUDA(cudaMemcpyAsync(counters, h, sizeof(h), cudaMemcpyHostToDevice, s));
     MI_CUDA(cudaStreamSynchronize(s));
     return LK_OK;
 }
@@ -382,25 +486,32 @@ int map_clear_outside(MapDevHost& mh, const int lo[3], const int hi[3], uint64_t
     if (e == cudaSuccess && n) e = cudaMemcpy(roots.data(), d_roots, (size_t)std::min(n, mh.n_roots) * sizeof(lk_map_root), cudaMemcpyDeviceToHost);
     if (e != cudaSuccess) { cudaFree(d_roots); cudaFree(d_cnt); cudaGetLastError(); err = cudaGetErrorString(e); return LK_ERR_CUDA; }
     n = std::min(n, mh.n_roots);
+    // kept roots first, dropped ones after them
+    std::vector<lk_map_root> gone;
     uint32_t keep = 0;
     for (uint32_t i = 0; i < n; ++i) {
         const lk_map_root& r = roots[i];
         const bool out = r.key[0] > hi[0] || r.key[0] < lo[0] || r.key[1] > hi[1] || r.key[1] < lo[1] || r.key[2] > hi[2] || r.key[2] < lo[2];
         if (!out) roots[keep++] = r;
+        else gone.push_back(r);
     }
     if (removed) *removed = n - keep;
     if (keep != n) {
+        std::copy(gone.begin(), gone.end(), roots.begin() + keep);
+        e = cudaMemcpyAsync(d_roots, roots.data(), (size_t)n * sizeof(lk_map_root), cudaMemcpyHostToDevice, s);
         k_hash_clear<<<(unsigned)((mh.hash_cap + 255) / 256), 256, 0, s>>>(mh.slots, mh.hash_cap);
-        if (keep) {
-            e = cudaMemcpyAsync(d_roots, roots.data(), (size_t)keep * sizeof(lk_map_root), cudaMemcpyHostToDevice, s);
-            k_hash_insert_roots<<<(keep + 255) / 256, 256, 0, s>>>(mh.slots, (uint32_t)(mh.hash_cap - 1), d_roots, keep, mh.counters + 2);
-        }
+        if (keep) k_hash_insert_roots<<<(keep + 255) / 256, 256, 0, s>>>(mh.slots, (uint32_t)(mh.hash_cap - 1), d_roots, keep, mh.counters + 2);
+        // their storage is recycled by the next launch that grows the map
+        k_free_subtrees<<<(n - keep + 127) / 128, 128, 0, s>>>(mh.dev(), d_roots + keep, n - keep, (int)mh.tile_slots);
         if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-        mh.n_roots = keep;
     }
     cudaFree(d_roots); cudaFree(d_cnt);
     if (e != cudaSuccess) { cudaGetLastError(); err = cudaGetErrorString(e); return LK_ERR_CUDA; }
-    return keep != n ? mh.push_counters(s, err) : LK_OK;
+    if (keep == n) return LK_OK;
+    rc = mh.sync_counters(s, err);  // the free lists as the kernel left them
+    if (rc) return rc;
+    mh.n_roots = keep;
+    return mh.push_counters(s, err);
 }
 
 int map_count_planes(MapDevHost& mh, uint64_t* planes, uint64_t* live_points, cudaStream_t s, std::string& err) {

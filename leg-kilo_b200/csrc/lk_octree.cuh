@@ -68,6 +68,25 @@ __device__ __forceinline__ void init_root_node(MapDev& md, const Globals& g, uin
     a->key[0] = kx; a->key[1] = ky; a->key[2] = kz;
 }
 
+// ---- free lists (MapDev::free_*) ---------------------------------------------------------------
+// An entry pushed during a launch stays pending until the host promotes it between launches (MapDevHost::push_counters),
+// so nothing freed by a launch is handed out again by the same launch: the warps of one launch that mutate different
+// roots, and the in-kernel insert across its grid barriers, keep the ordering they have with bump-only allocation.
+// Pops only read [0, avail), which no launch writes; a pop that finds the list empty leaves avail <= 0 (the host clamps).
+__device__ __forceinline__ bool free_pop(const MapDev& md, int l, uint32_t& v) {
+    const int a = atomicSub(reinterpret_cast<int*>(md.free_ctr + 3 * l), 1);
+    if (a <= 0) return false;
+    v = md.free_items[l][a - 1];
+    return true;
+}
+
+__device__ __forceinline__ void free_push(const MapDev& md, int l, uint32_t v) {
+    const uint32_t t = atomicAdd(md.free_ctr + 3 * l + 2, 1u);
+    if (t < md.free_cap[l]) md.free_items[l][t] = v;  // sized for twice the pool: never full in practice, a leak if so
+}
+
+__device__ __forceinline__ int std_tile(const Globals& g) { return even_up(g.max_points_num + 2); }
+
 // Bump-allocate `n` point slots (n even). Lane 0 only. Returns base or ~0ull on overflow.
 __device__ __forceinline__ unsigned long long alloc_points(MapDev& md, uint32_t n) {
     unsigned long long b = atomicAdd(md.n_points, (unsigned long long)n);
@@ -78,7 +97,25 @@ __device__ __forceinline__ unsigned long long alloc_points(MapDev& md, uint32_t 
     return b;
 }
 
+// `cap` point slots for one node: a standard tile comes off the free list when it holds one, anything else is bumped.
+__device__ __forceinline__ unsigned long long alloc_slots(MapDev& md, const Globals& g, int cap) {
+    uint32_t v;
+    if (cap == std_tile(g) && free_pop(md, FREE_TILES, v)) return v;
+    return alloc_points(md, (uint32_t)cap);
+}
+
+// Node `nd` will never read its points again (frozen leaf, cut parent): a standard tile goes back to the free list.
+// pts_cap keeps its value, so lk_map_download reports the node exactly as before; pts_base = NO_TILE says the tile
+// is gone (a slide must not return it twice). Lane 0 only.
+__device__ __forceinline__ void release_tile(MapDev& md, const Globals& g, uint32_t nd) {
+    MapAux* a = md.aux + nd;
+    if (a->pts_cap == std_tile(g) && a->pts_base != NO_TILE) free_push(md, FREE_TILES, a->pts_base);
+    a->pts_base = NO_TILE;
+}
+
 __device__ __forceinline__ int alloc_nodes8(MapDev& md) {
+    uint32_t v;
+    if (free_pop(md, FREE_GROUPS, v)) return (int)v;
     uint32_t b = atomicAdd(md.n_nodes, 8u);
     if (b + 8 > md.node_cap) {
         atomicOr(md.overflow, 1u);
@@ -100,7 +137,7 @@ __device__ inline bool retain_points(MapDev& md, const Globals& g, uint32_t nd, 
     if (in_pool) return true;
     int cap = even_up(max(cnt + 1, g.max_points_num + 2));
     unsigned long long base = 0;
-    if (lane == 0) base = alloc_points(md, (uint32_t)cap);
+    if (lane == 0) base = alloc_slots(md, g, cap);
     base = __shfl_sync(0xffffffffu, base, 0);
     if (base == ~0ull) return false;
     for (int j = lane; j < cnt; j += 32) copy_point(md.points + base + j, src + j);
@@ -146,12 +183,14 @@ __device__ inline int warp_cut(MapDev& md, const Globals& g, uint32_t nd, const 
 #pragma unroll
         for (int c = 0; c < 8; ++c) counts[c] += __popc(__ballot_sync(0xffffffffu, o == c));
     }
+    // a child of the standard size takes a tile of its own (recyclable); the larger ones share one bump block
+    const int tile = std_tile(g);
     int caps[8], offs[8], total = 0;
 #pragma unroll
     for (int c = 0; c < 8; ++c) {
         caps[c] = counts[c] > 0 ? even_up(max(counts[c] + 1, g.max_points_num + 2)) : 0;
         offs[c] = total;
-        total += caps[c];
+        if (caps[c] != tile) total += caps[c];
         cnt_out[c] = counts[c];
     }
     int cbase = -1;
@@ -159,11 +198,25 @@ __device__ inline int warp_cut(MapDev& md, const Globals& g, uint32_t nd, const 
     if (lane == 0) {
         cbase = md.nodes[nd].child_base;
         if (cbase < 0) cbase = alloc_nodes8(md);
-        pbase = (cbase >= 0) ? alloc_points(md, (uint32_t)total) : ~0ull;
+        pbase = (cbase >= 0 && total > 0) ? alloc_points(md, (uint32_t)total) : 0;
     }
     cbase = __shfl_sync(0xffffffffu, cbase, 0);
     pbase = __shfl_sync(0xffffffffu, pbase, 0);
     if (cbase < 0 || pbase == ~0ull) return -1;
+    bool mine = false;  // lane c < 8 allocates child c's own tile
+#pragma unroll
+    for (int c = 0; c < 8; ++c) mine |= lane == c && caps[c] == tile;
+    unsigned long long own = mine ? alloc_slots(md, g, tile) : 0;
+    bool failed = false;
+    unsigned long long cpb[8], my_pb = 0;  // first slot of each child's points; lane c < 8: child c's
+#pragma unroll
+    for (int c = 0; c < 8; ++c) {
+        const unsigned long long t = __shfl_sync(0xffffffffu, own, c);
+        cpb[c] = (caps[c] == tile) ? t : pbase + offs[c];
+        failed |= cpb[c] == ~0ull;
+        if (lane == c) my_pb = cpb[c];
+    }
+    if (failed) return -1;
     int run[8];
 #pragma unroll
     for (int c = 0; c < 8; ++c) run[c] = 0;
@@ -174,7 +227,7 @@ __device__ inline int warp_cut(MapDev& md, const Globals& g, uint32_t nd, const 
 #pragma unroll
         for (int c = 0; c < 8; ++c) {
             uint32_t m = __ballot_sync(0xffffffffu, o == c);
-            if (o == c) copy_point(md.points + pbase + offs[c] + run[c] + __popc(m & lt), src + j);
+            if (o == c) copy_point(md.points + cpb[c] + run[c] + __popc(m & lt), src + j);
             run[c] += __popc(m);
         }
     }
@@ -186,7 +239,7 @@ __device__ inline int warp_cut(MapDev& md, const Globals& g, uint32_t nd, const 
         if (!existed) {
             init_child_node(md, nd, child, c);
             MapAux* a = md.aux + child;
-            a->pts_base = (uint32_t)(pbase + offs[c]);
+            a->pts_base = (uint32_t)my_pb;
             a->pts_count = counts[c];
             a->pts_cap = caps[c];
             a->new_points = counts[c];  // new_points_++ per pushed point (:159)
@@ -240,6 +293,7 @@ __device__ inline void warp_init_octo_tree(MapDev& md, const Globals& g, WarpTil
                         md.nodes[nd].flags = (flags0 | LK_NODE_IS_PLANE | LK_NODE_INIT_OCTO) & ~LK_NODE_UPDATE_ENABLE;
                         md.aux[nd].pts_count = 0;
                         md.aux[nd].new_points = 0;
+                        if (in_pool) release_tile(md, g, nd);
                     }
                 } else {
                     retain_points(md, g, nd, src, cnt, in_pool, lane);
@@ -262,6 +316,8 @@ __device__ inline void warp_init_octo_tree(MapDev& md, const Globals& g, WarpTil
                         md.nodes[nd].flags = (md.nodes[nd].flags | LK_NODE_INIT_OCTO) & ~LK_NODE_IS_PLANE;
                         md.aux[nd].pts_count = 0;  // the parent never looks at its own points again
                         md.aux[nd].new_points = 0;
+                        // warp_cut copied them out before its last __syncwarp; the bulk build's sorted scratch is no tile
+                        if (in_pool && cbase >= 0) release_tile(md, g, nd);
                     }
                     if (cbase >= 0) {
                         const int thr_c = g.layer_init_num[layer + 1 < 5 ? layer + 1 : 4];
@@ -284,8 +340,8 @@ __device__ inline void warp_append(MapDev& md, const Globals& g, uint32_t nd, co
     if (lane == 0) {
         MapAux* a = md.aux + nd;
         if (a->pts_cap == 0) {
-            int cap = even_up(g.max_points_num + 2);
-            unsigned long long b = alloc_points(md, (uint32_t)cap);
+            const int cap = std_tile(g);
+            unsigned long long b = alloc_slots(md, g, cap);
             if (b != ~0ull) {
                 a->pts_base = (uint32_t)b;
                 a->pts_cap = cap;
@@ -345,6 +401,7 @@ __device__ inline void warp_update_octo_tree(MapDev& md, const Globals& g, WarpT
                     md.nodes[nd].flags &= ~LK_NODE_UPDATE_ENABLE;
                     md.aux[nd].pts_count = 0;
                     md.aux[nd].new_points = 0;
+                    release_tile(md, g, nd);  // the points are dropped (:206): update_enable is off for good
                 }
             }
             return;

@@ -32,7 +32,16 @@ struct MapDev {
     unsigned long long* n_points;  // bump allocator of point slots
     uint32_t* n_roots;
     uint32_t* overflow;  // bit0 nodes, bit1 points, bit2 hash
+    // Free lists of recycled storage (lk_octree.cuh: free_pop / free_push): standard point tiles (their first slot),
+    // 8-node child groups (their first node) and single root nodes. free_ctr[3 l .. 3 l + 2] = avail | base | top of
+    // list l: [0, avail) may be popped, pushes land at [top, ...), and the host promotes [base, top) between launches.
+    uint32_t* free_items[3];
+    uint32_t free_cap[3];
+    uint32_t* free_ctr;
 };
+
+enum { FREE_TILES = 0, FREE_GROUPS = 1, FREE_SINGLES = 2 };
+constexpr uint32_t NO_TILE = 0xffffffffu;  // aux.pts_base of a node whose tile went back to the free list
 
 constexpr int TILE_PTS = 64;  // points per staged tile (5 120 B)
 

@@ -52,6 +52,7 @@ def lib():
         L.lk_map_build.argtypes = [vp, vp, vp, C.c_size_t, vp, vp, vp]
         L.lk_map_stats.argtypes = [vp, vp]
         L.lk_map_slide.argtypes = [vp, vp, vp, vp]
+        L.lk_map_memory.argtypes = [vp, vp]
         L.lk_tum_line.argtypes = [dbl, vp, vp, C.c_char_p, C.c_size_t]
         L.lk_scan_update.argtypes = [vp, i32] + [vp] * 9 + [i32, i32, vp, vp]
         L.lk_batch_stage.argtypes = [vp, i32] + [vp] * 9
@@ -188,6 +189,13 @@ class Engine:
         out = np.zeros(4, np.uint64)
         self._chk(lib().lk_map_stats(self.h, _p(out)))
         return dict(roots=int(out[0]), nodes=int(out[1]), points=int(out[2]), planes=int(out[3]))
+
+    def map_memory(self):
+        """lk_map_memory: bump-allocated and free-listed nodes / point slots, pool bytes, pool reallocations."""
+        out = np.zeros(6, np.uint64)
+        self._chk(lib().lk_map_memory(self.h, _p(out)))
+        return dict(nodes=int(out[0]), free_nodes=int(out[1]), point_slots=int(out[2]), free_point_slots=int(out[3]),
+                    pool_bytes=int(out[4]), reallocs=int(out[5]))
 
     # ---- hot path ------------------------------------------------------------------------------
     @staticmethod
