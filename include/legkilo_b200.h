@@ -364,6 +364,62 @@ int lk_decode_pointcloud2(lk_handle h, const uint8_t* data, uint32_t n_points, c
 int lk_preprocess_scan(lk_handle h, const float* pts_in, uint32_t n_in, float leaf_size, float* pts_out,
                        uint32_t* n_out, uint32_t* bucket_offsets, float* bucket_curvature, uint32_t* n_buckets);
 
+/* ---- leg kinematics: what feeds lk_obs_kinimu / the kin queue of lk_process_scan ----------- */
+
+/* = legkilo::Kinematics::Config (kinematics.h:27-35), same field order. */
+typedef struct lk_leg_cfg {
+    double leg_offset_x;
+    double leg_offset_y;
+    double leg_calf_length;
+    double leg_thigh_length;
+    double leg_thigh_offset;
+    double contact_force_threshold_up;   /* ContactDetector T_on_ */
+    double contact_force_threshold_down; /* ContactDetector T_off_ */
+} lk_leg_cfg; /* 56 B */
+
+/* The fields of one unitree_legged_msgs::HighState that Kinematics::processing and the redundancy check read, in the
+ * MESSAGE's index order (legs FL FR RL RR, kinematics.cc:13-16) and the message's own types. */
+typedef struct lk_leg_state {
+    double stamp;           /* stamp.toSec() */
+    float acc[3];           /* imu.accelerometer */
+    float gyr[3];           /* imu.gyroscope */
+    float q[12];            /* motorState[0..11].q: hip, thigh, calf of FL, FR, RL, RR */
+    float dq[12];           /* motorState[0..11].dq */
+    int16_t foot_force[4];  /* footForce (FL FR RL RR) */
+} lk_leg_state; /* 136 B */
+
+/* What a caller carries from one lk_leg_kinematics call to the next (like lk_stream_clock): the four
+ * ContactDetector states (kinematics.h:10-23) in the project's leg order FR FL RR RL, and imu.accelerometer[2] /
+ * imu.gyroscope[2] of the last RAW message, kept or dropped (ros_interface.cc:222, :228, :247). */
+typedef struct lk_leg_track {
+    int32_t in_contact[4];
+    float last_acc_z;
+    float last_gyr_z;
+} lk_leg_track; /* 24 B */
+
+/* The reference's initial state: every detector in contact (kinematics.h:12), the previous message zero-initialised
+ * (the static HighState of ros_interface.cc:222). Host-side helper. */
+int lk_leg_track_default(lk_leg_track* t);
+
+/* RosInterface::kinematicImuCallBack (ros_interface.cc:221-248) without its ROS plumbing, over `n` consecutive
+ * messages, then Kinematics::processing (kinematics.cc:5-90) on every message it keeps:
+ *  - redundancy != 0 drops a message whose imu.accelerometer[2] AND imu.gyroscope[2] both equal (float ==) those of
+ *    the previous raw message (ros_interface.cc:225-231); for in[0] that is track_inout's last_acc_z / last_gyr_z.
+ *    A dropped message does not advance the contact detectors.
+ *  - contact: the detector of leg FR / FL / RR / RL reads footForce[1] / [0] / [3] / [2] (kinematics.cc:17-20) and
+ *    switches on when out of contact and force > threshold_up, off when in contact and force < threshold_down.
+ *  - foot_pos / foot_vel: forward kinematics and Jacobian times joint rates in fp64 (caculateFootPosVel,
+ *    kinematics.cc:54-90), joints of FR / FL / RR / RL from motorState[3..5] / [0..2] / [9..11] / [6..8].
+ * The kept samples are written in order to out[0 .. *n_out) (capacity n) and the updated track is written back.
+ * n == 0 returns LK_OK with *n_out = 0 and the track unchanged. A NULL h, cfg, track_inout or n_out, a NULL in / out
+ * with n > 0, or a non-finite cfg field is LK_ERR_INVALID_ARG.
+ * Runs on the device for any n: one thread per message, two device-wide scans (output positions; the contact
+ * detectors as a composition of per-message transfer functions), one thread per kept message. n_out, stamps,
+ * contacts, acc, gyr and the track are bitwise what the reference computes; foot_pos / foot_vel can differ from a CPU
+ * build by a few ulp (device sin / cos against the host libm, and FMA contraction by nvcc). */
+int lk_leg_kinematics(lk_handle h, const lk_leg_cfg* cfg, const lk_leg_state* in, uint32_t n, int32_t redundancy,
+                      lk_leg_track* track_inout, lk_kinimu_meas* out, uint32_t* n_out);
+
 #ifdef __cplusplus
 }
 #endif

@@ -18,6 +18,10 @@ int decode_pointcloud2_device(const uint8_t* h_data, uint32_t n, const lk_pc2_la
 int preprocess_scan_device(const float* h_pts_in, uint32_t n, float leaf, float* h_pts_out, uint32_t* n_out,
                            uint32_t* h_bucket_offsets, float* h_bucket_curv, uint32_t* n_buckets, cudaStream_t s,
                            std::string& err);
+size_t leg_kinematics_scratch_bytes(uint32_t n);
+int leg_kinematics_device(const lk_leg_cfg& cfg, const lk_leg_state* h_in, uint32_t n, int redundancy,
+                          lk_leg_track* track, lk_kinimu_meas* h_out, uint32_t* n_out, void* scratch, cudaStream_t s,
+                          std::string& err);
 }  // namespace lk
 
 using namespace lk;
@@ -124,6 +128,7 @@ struct lk_context {
     float4* direct_world = nullptr;
     double hprof[8] = {0, 0, 0, 0, 0, 0, 0, 0};  // host-side ns of lk_scan_update: stage | enqueue | wait+fetch | calls
     DevBuf Qc;                     // process noise kept on the device between calls
+    DevBuf leg_scratch;            // lk_leg_kinematics: inputs, flags, scans and outputs of the last call's size
     std::vector<double> Q_shadow;  // what Qc holds
 
     // timing
@@ -328,6 +333,7 @@ int lk_destroy(lk_handle h) {
                       &h->ins_counters, &h->ins_list, &h->fb_list, &h->fb_cnt};
     for (DevBuf* b : bufs) b->release();
     h->h_small_in.release();
+    h->leg_scratch.release();
     h->h_small_out.release();
     for (cudaEvent_t e : h->kev) cudaEventDestroy(e);
     if (h->ev0) cudaEventDestroy(h->ev0);
@@ -353,6 +359,14 @@ int lk_state_default(lk_state* x) {
     std::memset(x, 0, sizeof(*x));
     x->rot[0] = x->rot[4] = x->rot[8] = 1.0;
     x->grav[2] = -9.81;
+    return LK_OK;
+}
+
+int lk_leg_track_default(lk_leg_track* t) {
+    if (!t) return LK_ERR_INVALID_ARG;
+    for (int k = 0; k < 4; ++k) t->in_contact[k] = 1;  // ContactDetector::in_contact_{true} (kinematics.h:12)
+    t->last_acc_z = 0.0f;                                // the zero-initialised static HighState (ros_interface.cc:222)
+    t->last_gyr_z = 0.0f;
     return LK_OK;
 }
 
@@ -1404,6 +1418,23 @@ int lk_preprocess_scan(lk_handle h, const float* pts_in, uint32_t n_in, float le
     h->prev_fused = false;
     std::string err;
     int rc = preprocess_scan_device(pts_in, n_in, leaf_size, pts_out, n_out, bucket_offsets, bucket_curvature, n_buckets, h->stream, err);
+    return rc ? fail(h, rc, err) : LK_OK;
+}
+
+int lk_leg_kinematics(lk_handle h, const lk_leg_cfg* cfg, const lk_leg_state* in, uint32_t n, int32_t redundancy,
+                      lk_leg_track* track_inout, lk_kinimu_meas* out, uint32_t* n_out) {
+    if (!h || !cfg || !track_inout || !n_out || (n && (!in || !out))) return fail(h, LK_ERR_INVALID_ARG, "null argument");
+    const double f[7] = {cfg->leg_offset_x,     cfg->leg_offset_y,     cfg->leg_calf_length,           cfg->leg_thigh_length,
+                         cfg->leg_thigh_offset, cfg->contact_force_threshold_up, cfg->contact_force_threshold_down};
+    for (double v : f)
+        if (!std::isfinite(v)) return fail(h, LK_ERR_INVALID_ARG, "non-finite leg configuration");
+    *n_out = 0;
+    if (!n) return LK_OK;
+    cudaSetDevice(h->device);
+    h->prev_fused = false;
+    LK_CUDA(h, h->leg_scratch.ensure(leg_kinematics_scratch_bytes(n)));
+    std::string err;
+    int rc = leg_kinematics_device(*cfg, in, n, redundancy, track_inout, out, n_out, h->leg_scratch.p, h->stream, err);
     return rc ? fail(h, rc, err) : LK_OK;
 }
 

@@ -72,6 +72,8 @@ def lib():
                                       vp, vp]
         L.lk_decode_pointcloud2.argtypes = [vp, vp, u32, vp, C.c_float, i32, dbl, vp, vp, vp, vp, vp]
         L.lk_preprocess_scan.argtypes = [vp, vp, u32, C.c_float, vp, vp, vp, vp, vp]
+        L.lk_leg_track_default.argtypes = [vp]
+        L.lk_leg_kinematics.argtypes = [vp, vp, vp, u32, i32, vp, vp, vp]
         _LIB = L
     return _LIB
 
@@ -343,6 +345,23 @@ class Engine:
         no = np.zeros(1, np.uint32); nb = np.zeros(1, np.uint32)
         self._chk(lib().lk_preprocess_scan(self.h, _p(pts), n, leaf, _p(out), _p(no), _p(offs), _p(curv), _p(nb)))
         return out[:no[0]].copy(), offs[:nb[0] + 1].copy(), curv[:nb[0]].copy()
+
+    def leg_kinematics(self, states, cfg, track=None, redundancy=True):
+        """lk_leg_kinematics: unitree HighState fields (abi.LEG_STATE_DTYPE) -> kinematic-inertial samples
+        (abi.KINIMU_DTYPE), the redundancy drop and the contact detectors carried by `track` (abi.LkLegTrack; None =
+        the reference's initial state). `cfg` is a configuration dict or an abi.LkLegCfg. Returns (kin, new track)."""
+        states = np.ascontiguousarray(states, abi.LEG_STATE_DTYPE)
+        lc = cfg if isinstance(cfg, abi.LkLegCfg) else abi.leg_cfg(cfg)
+        tr = abi.LkLegTrack()
+        if track is None:
+            self._chk(lib().lk_leg_track_default(C.byref(tr)))
+        else:
+            C.memmove(C.byref(tr), C.byref(track), C.sizeof(tr))
+        out = np.zeros(len(states), abi.KINIMU_DTYPE)
+        no = C.c_uint32(0)
+        self._chk(lib().lk_leg_kinematics(self.h, C.byref(lc), _p(states), len(states), int(bool(redundancy)), C.byref(tr),
+                                          _p(out), C.byref(no)))
+        return out[:no.value].copy(), tr
 
     def predict(self, x, P, Q, dt, prop_state=True, prop_cov=True):
         x = np.array(x, abi.STATE_DTYPE, copy=True); batch = len(x)

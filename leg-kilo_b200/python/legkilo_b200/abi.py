@@ -45,6 +45,21 @@ class LkKinImuMeas(C.Structure):
                 ("contact", C.c_int32 * 4), ("acc", C.c_double * 3), ("gyr", C.c_double * 3)]
 
 
+class LkLegCfg(C.Structure):
+    _fields_ = [(n, C.c_double) for n in (
+        "leg_offset_x", "leg_offset_y", "leg_calf_length", "leg_thigh_length", "leg_thigh_offset",
+        "contact_force_threshold_up", "contact_force_threshold_down")]
+
+
+class LkLegTrack(C.Structure):
+    _fields_ = [("in_contact", C.c_int32 * 4), ("last_acc_z", C.c_float), ("last_gyr_z", C.c_float)]
+
+
+def leg_track_default() -> LkLegTrack:
+    """lk_leg_track_default: every detector in contact, a zero previous message (kinematics.h:12, ros_interface.cc:222)."""
+    return LkLegTrack((C.c_int32 * 4)(1, 1, 1, 1), 0.0, 0.0)
+
+
 class LkPc2Layout(C.Structure):
     _fields_ = [("point_step", C.c_uint32), ("off_x", C.c_uint32), ("off_y", C.c_uint32), ("off_z", C.c_uint32),
                 ("off_intensity", C.c_uint32), ("off_time", C.c_uint32), ("lidar_type", C.c_int32), ("reserved", C.c_int32)]
@@ -76,7 +91,11 @@ CLOCK_DTYPE = np.dtype([("last_predict_time", "f8"), ("last_update_time", "f8")]
 IMU_DTYPE = np.dtype([("stamp", "f8"), ("acc", "f8", (3,)), ("gyr", "f8", (3,))])
 KINIMU_DTYPE = np.dtype([("stamp", "f8"), ("foot_pos", "f8", (4, 3)), ("foot_vel", "f8", (4, 3)),
                          ("contact", "i4", (4,)), ("acc", "f8", (3,)), ("gyr", "f8", (3,))])
+# lk_leg_state: one unitree_legged_msgs::HighState, message index order (legs FL FR RL RR) and types
+LEG_STATE_DTYPE = np.dtype([("stamp", "f8"), ("acc", "f4", (3,)), ("gyr", "f4", (3,)), ("q", "f4", (12,)),
+                            ("dq", "f4", (12,)), ("foot_force", "i2", (4,))], align=True)
 assert STATE_DTYPE.itemsize == C.sizeof(LkState) == 288
+assert LEG_STATE_DTYPE.itemsize == 136 and C.sizeof(LkLegCfg) == 56 and C.sizeof(LkLegTrack) == 24
 assert KINIMU_DTYPE.itemsize == C.sizeof(LkKinImuMeas)
 
 # map blob dtypes (include/legkilo_b200.h)
@@ -131,19 +150,25 @@ _COMMON = dict(
     chd_meas_noise=0.1, contact_meas_noise=0.001, lidar_point_meas_ratio=10.0,
     max_layer=2, voxel_size=0.5, min_eigen_value=0.01, sigma_num=3.0, beam_err=0.2, dept_err=0.04,
     layer_init_num=(5, 5, 5, 5, 5), max_points_num=50, map_sliding_en=0, half_map_size=100, sliding_thresh=8.0,
-    gravity=9.81, blind=1.5, filter_num=3)
+    gravity=9.81, blind=1.5, filter_num=3, redundancy=True)
+
+# Kinematics::Config (legkilo/config/*.yaml:45-51)
+_LEG_UNITREE = dict(leg_offset_x=0.1881, leg_offset_y=0.04675, leg_calf_length=0.213, leg_thigh_length=0.213,
+                    leg_thigh_offset=0.08, contact_force_threshold_up=220.0, contact_force_threshold_down=200.0)
+_LEG_DITER = dict(leg_offset_x=0.1934, leg_offset_y=0.0465, leg_calf_length=0.213, leg_thigh_length=0.213,
+                  leg_thigh_offset=0.0465, contact_force_threshold_up=40.0, contact_force_threshold_down=60.0)
 
 CONFIGS = {
-    "leg_fusion": dict(_COMMON, only_imu_use=False, extrinsic_T=(0.0, 0.0, 0.20),
+    "leg_fusion": dict(_COMMON, **_LEG_UNITREE, only_imu_use=False, extrinsic_T=(0.0, 0.0, 0.20),
                        extrinsic_R=(1, 0, 0, 0, 1, 0, 0, 0, 1), voxel_grid_resolution=0.3, lidar_type=1, time_scale=1.0,
                        imu_acc_meas_noise=0.1, imu_acc_z_meas_noise=1.0, imu_gyr_meas_noise=0.01),
-    "diter": dict(_COMMON, only_imu_use=False, extrinsic_T=(0.005, 0.00056, 0.299),
+    "diter": dict(_COMMON, **_LEG_DITER, only_imu_use=False, extrinsic_T=(0.005, 0.00056, 0.299),
                   extrinsic_R=(1, 0, 0, 0, 1, 0, 0, 0, 1), voxel_grid_resolution=0.5, lidar_type=2, time_scale=1e-9,
                   imu_acc_meas_noise=0.01, imu_acc_z_meas_noise=0.1, imu_gyr_meas_noise=0.001),
-    "hilti": dict(_COMMON, only_imu_use=True, extrinsic_T=(-0.001, -0.00855, 0.055),
+    "hilti": dict(_COMMON, **_LEG_UNITREE, only_imu_use=True, extrinsic_T=(-0.001, -0.00855, 0.055),
                   extrinsic_R=(0, -1, 0, -1, 0, 0, 0, 0, -1), voxel_grid_resolution=0.5, lidar_type=3, time_scale=1.0,
                   imu_acc_meas_noise=0.01, imu_acc_z_meas_noise=0.01, imu_gyr_meas_noise=0.01, blind=0.2),
-    "nclt": dict(_COMMON, only_imu_use=True, extrinsic_T=(0.0, 0.0, 0.28), extrinsic_R=(1, 0, 0, 0, 1, 0, 0, 0, 1),
+    "nclt": dict(_COMMON, **_LEG_UNITREE, only_imu_use=True, extrinsic_T=(0.0, 0.0, 0.28), extrinsic_R=(1, 0, 0, 0, 1, 0, 0, 0, 1),
                  voxel_grid_resolution=0.5, lidar_type=1, time_scale=1e-6, imu_acc_meas_noise=0.1,
                  imu_acc_z_meas_noise=1.0, imu_gyr_meas_noise=0.01),
 }
@@ -154,6 +179,14 @@ def eskf_cfg(cfg: dict) -> LkEskfCfg:
     for name, _ in LkEskfCfg._fields_:
         setattr(e, name, float(cfg[name]))
     return e
+
+
+def leg_cfg(cfg: dict) -> LkLegCfg:
+    """Kinematics::Config (kinematics.h:27-35) of a dataset configuration."""
+    c = LkLegCfg()
+    for name, _ in LkLegCfg._fields_:
+        setattr(c, name, float(cfg[name]))
+    return c
 
 
 def map_cfg(cfg: dict) -> LkMapCfg:

@@ -260,3 +260,51 @@ def kinimu_stream(t0: float, t1: float, rate_hz: float = 400.0, stream: int = 43
     pat = np.array([[1, 0, 0, 1], [0, 1, 1, 0], [1, 1, 1, 1]], np.int32)
     m["contact"] = pat[phase]
     return m
+
+
+def leg_state_stream(t0: float, t1: float, rate_hz: float = 500.0, cfg_name: str = "leg_fusion", stream: int = 47):
+    """unitree HighState fields (abi.LEG_STATE_DTYPE, message order FL FR RL RR) on (t0, t1] for lk_leg_kinematics:
+    joints around a standing pose with a 2 Hz trot (diagonal pairs FL+RR / FR+RL in antiphase), dq the derivative plus
+    noise; foot forces that cross both contact thresholds of `cfg_name`, sit between them for stretches and hit each
+    exactly now and then; runs of messages that repeat the previous accelerometer z AND gyroscope z (dropped by the
+    redundancy check), and some that repeat only one of them (kept)."""
+    from . import abi
+    cfg = abi.CONFIGS[cfg_name]
+    g = rng(stream)
+    n = int(np.floor((t1 - t0) * rate_hz))
+    m = np.zeros(n, abi.LEG_STATE_DTYPE)
+    t = t0 + (np.arange(n) + 1) / rate_hz
+    m["stamp"] = t
+    w = 2.0 * np.pi * 2.0
+    phase = w * t[:, None] + np.array([0.0, np.pi, np.pi, 0.0])[None]  # (n, 4)
+    stand = np.array([0.0, 0.8, -1.6]); amp = np.array([0.05, 0.25, 0.35])
+    q = stand + amp * np.sin(phase)[:, :, None]
+    dq = amp * w * np.cos(phase)[:, :, None] + 0.05 * g.standard_normal((n, 4, 3))
+    m["q"] = q.reshape(n, 12).astype(np.float32)
+    m["dq"] = dq.reshape(n, 12).astype(np.float32)
+    up, down = cfg["contact_force_threshold_up"], cfg["contact_force_threshold_down"]
+    lo, hi = min(up, down), max(up, down)
+    # stance (sin < 0) well above both thresholds, swing well below, a trapezoid so that the crossing takes a few samples
+    mid, half = 0.5 * (lo + hi), 0.5 * (hi - lo) + 60.0
+    f = mid + half * np.clip(-2.5 * np.sin(phase), -1.0, 1.0) + 4.0 * g.standard_normal((n, 4))
+    # stretches of 10-40 samples strictly between the thresholds
+    for leg in range(4):
+        for s0 in g.integers(0, max(n, 1), size=max(n // 150, 1)):
+            seg = f[s0:s0 + int(g.integers(10, 41)), leg]
+            seg[:] = g.uniform(lo + 1.0, hi - 1.0, size=len(seg))
+    hit = g.uniform(size=(n, 4))
+    f = np.where(hit < 0.02, up, np.where(hit > 0.98, down, f))
+    m["foot_force"] = np.clip(np.rint(f), -32768, 32767).astype(np.int16)
+    acc = (np.array([0.15, -0.1, 9.79]) + 0.05 * g.standard_normal((n, 3))).astype(np.float32)
+    gyr = (np.array([0.01, -0.02, 0.12]) + 0.005 * g.standard_normal((n, 3))).astype(np.float32)
+    # repeats: each message copies the previous one's z pair with probability 0.3, so runs form
+    rep = g.uniform(size=n) < 0.3
+    rep[0] = False
+    src = np.maximum.accumulate(np.where(rep, 0, np.arange(n)))
+    acc[:, 2] = acc[src, 2]; gyr[:, 2] = gyr[src, 2]
+    one = (~rep) & (g.uniform(size=n) < 0.05)  # only the accelerometer z repeats: not redundant
+    one[0] = False
+    prev = np.flatnonzero(one) - 1
+    acc[one, 2] = acc[prev, 2]
+    m["acc"] = acc; m["gyr"] = gyr
+    return m
