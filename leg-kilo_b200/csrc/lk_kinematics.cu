@@ -12,6 +12,7 @@
 #include <string>
 
 #include "lk_device.cuh"
+#include "lk_host.h"
 
 namespace lk {
 
@@ -134,16 +135,6 @@ struct LegScratch {  // one device block, carved in this order
 
 size_t leg_kinematics_scratch_bytes(uint32_t n) { return n ? LegScratch(n).total : 0; }
 
-#define LEG_CUDA(expr)                                                                    \
-    do {                                                                                  \
-        cudaError_t e__ = (expr);                                                         \
-        if (e__ != cudaSuccess) {                                                         \
-            cudaGetLastError();                                                           \
-            err = std::string(#expr) + ": " + cudaGetErrorString(e__);                    \
-            return e__ == cudaErrorMemoryAllocation ? LK_ERR_OUT_OF_MEMORY : LK_ERR_CUDA; \
-        }                                                                                 \
-    } while (0)
-
 // `scratch` holds leg_kinematics_scratch_bytes(n) bytes of device memory. n > 0.
 int leg_kinematics_device(const lk_leg_cfg& cfg, const lk_leg_state* h_in, uint32_t n, int redundancy,
                           lk_leg_track* track, lk_kinimu_meas* h_out, uint32_t* n_out, void* scratch, cudaStream_t s,
@@ -159,23 +150,23 @@ int leg_kinematics_device(const lk_leg_cfg& cfg, const lk_leg_state* h_in, uint3
     auto* d_res = reinterpret_cast<LegResult*>(base + L.res);
     void* d_tmp = base + L.tmp;
     size_t tb = L.total - L.tmp;
-    LEG_CUDA(cudaMemcpyAsync(d_in, h_in, (size_t)n * sizeof(lk_leg_state), cudaMemcpyHostToDevice, s));
+    LK_CUDA(err, cudaMemcpyAsync(d_in, h_in, (size_t)n * sizeof(lk_leg_state), cudaMemcpyHostToDevice, s));
     const unsigned g = (n + 255) / 256;
     k_leg_flags<<<g, 256, 0, s>>>(d_in, n, redundancy, track->last_acc_z, track->last_gyr_z,
                                   cfg.contact_force_threshold_up, cfg.contact_force_threshold_down, d_keep, d_code);
-    LEG_CUDA(cub::DeviceScan::ExclusiveSum(d_tmp, tb, d_keep, d_pos, (int)n, s));
+    LK_CUDA(err, cub::DeviceScan::ExclusiveSum(d_tmp, tb, d_keep, d_pos, (int)n, s));
     tb = L.total - L.tmp;
-    LEG_CUDA(cub::DeviceScan::InclusiveScan(d_tmp, tb, d_code, d_scode, LegCompose(), (int)n, s));
+    LK_CUDA(err, cub::DeviceScan::InclusiveScan(d_tmp, tb, d_code, d_scode, LegCompose(), (int)n, s));
     const int4 c0 = make_int4(track->in_contact[0] != 0, track->in_contact[1] != 0, track->in_contact[2] != 0,
                               track->in_contact[3] != 0);
     k_leg_scatter<<<g, 256, 0, s>>>(d_in, n, cfg, c0, d_keep, d_pos, d_scode, d_out, d_res);
-    LEG_CUDA(cudaGetLastError());
+    LK_CUDA(err, cudaGetLastError());
     LegResult r;
-    LEG_CUDA(cudaMemcpyAsync(&r, d_res, sizeof(r), cudaMemcpyDeviceToHost, s));
-    LEG_CUDA(cudaStreamSynchronize(s));
+    LK_CUDA(err, cudaMemcpyAsync(&r, d_res, sizeof(r), cudaMemcpyDeviceToHost, s));
+    LK_CUDA(err, cudaStreamSynchronize(s));
     if (r.n_out)
-        LEG_CUDA(cudaMemcpyAsync(h_out, d_out, (size_t)r.n_out * sizeof(lk_kinimu_meas), cudaMemcpyDeviceToHost, s));
-    LEG_CUDA(cudaStreamSynchronize(s));
+        LK_CUDA(err, cudaMemcpyAsync(h_out, d_out, (size_t)r.n_out * sizeof(lk_kinimu_meas), cudaMemcpyDeviceToHost, s));
+    LK_CUDA(err, cudaStreamSynchronize(s));
     *n_out = r.n_out;
     for (int leg = 0; leg < 4; ++leg) track->in_contact[leg] = r.in_contact[leg];
     track->last_acc_z = r.last_acc_z;

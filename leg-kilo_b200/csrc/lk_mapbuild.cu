@@ -149,46 +149,32 @@ int map_build_device(MapDevHost& mh, const Globals& g, const float* d_xyz_world,
         bc.Crot[i] = rot_cov[i];
         bc.Cpos[i] = pos_cov[i];
     }
-#define MB_CUDA(expr)                                                           \
-    do {                                                                        \
-        cudaError_t e__ = (expr);                                               \
-        if (e__ != cudaSuccess) {                                               \
-            cudaGetLastError();                                                 \
-            err = std::string(#expr) + ": " + cudaGetErrorString(e__);          \
-            return e__ == cudaErrorMemoryAllocation ? LK_ERR_OUT_OF_MEMORY : LK_ERR_CUDA; \
-        }                                                                       \
-    } while (0)
-
-    unsigned long long *keys = nullptr, *keys_sorted = nullptr, *ukeys = nullptr;
-    uint32_t *idx = nullptr, *idx_sorted = nullptr, *counts = nullptr, *starts = nullptr, *nruns = nullptr, *bad = nullptr;
-    DevPoint *recs = nullptr, *sorted = nullptr;
-    void* tmp = nullptr;
-    size_t tmp_bytes = 0;
-    auto cleanup = [&]() {
-        void* ptrs[] = {keys, keys_sorted, ukeys, idx, idx_sorted, counts, starts, nruns, bad, recs, sorted, tmp};
-        for (void* p : ptrs)
-            if (p) cudaFree(p);
-    };
     const size_t nn = std::max<size_t>(n, 1);
+    DevBuf b_keys, b_keys_sorted, b_ukeys, b_idx, b_idx_sorted, b_counts, b_starts, b_nruns, b_bad, b_recs, b_sorted, b_tmp;
+    LK_CUDA(err, b_keys.alloc(nn * 8));
+    LK_CUDA(err, b_keys_sorted.alloc(nn * 8));
+    LK_CUDA(err, b_ukeys.alloc(nn * 8));
+    LK_CUDA(err, b_idx.alloc(nn * 4));
+    LK_CUDA(err, b_idx_sorted.alloc(nn * 4));
+    LK_CUDA(err, b_counts.alloc(nn * 4));
+    LK_CUDA(err, b_starts.alloc(nn * 4));
+    LK_CUDA(err, b_nruns.alloc(16));
+    LK_CUDA(err, b_bad.alloc(16));
+    LK_CUDA(err, b_recs.alloc(nn * sizeof(DevPoint)));
+    LK_CUDA(err, b_sorted.alloc(nn * sizeof(DevPoint)));
+    auto* keys = b_keys.as<unsigned long long>();
+    auto* keys_sorted = b_keys_sorted.as<unsigned long long>();
+    auto* ukeys = b_ukeys.as<unsigned long long>();
+    auto* idx = b_idx.as<uint32_t>();
+    auto* idx_sorted = b_idx_sorted.as<uint32_t>();
+    auto* counts = b_counts.as<uint32_t>();
+    auto* starts = b_starts.as<uint32_t>();
+    auto* nruns = b_nruns.as<uint32_t>();
+    auto* bad = b_bad.as<uint32_t>();
+    auto* recs = b_recs.as<DevPoint>();
+    auto* sorted = b_sorted.as<DevPoint>();
+    size_t tmp_bytes = 0;
     cudaError_t e;
-#define MB_ALLOC(ptr, bytes)                                   \
-    if ((e = cudaMalloc((void**)&ptr, (bytes))) != cudaSuccess) { \
-        cleanup();                                             \
-        cudaGetLastError();                                    \
-        err = "cudaMalloc failed in lk_map_build";             \
-        return LK_ERR_OUT_OF_MEMORY;                           \
-    }
-    MB_ALLOC(keys, nn * 8);
-    MB_ALLOC(keys_sorted, nn * 8);
-    MB_ALLOC(ukeys, nn * 8);
-    MB_ALLOC(idx, nn * 4);
-    MB_ALLOC(idx_sorted, nn * 4);
-    MB_ALLOC(counts, nn * 4);
-    MB_ALLOC(starts, nn * 4);
-    MB_ALLOC(nruns, 16);
-    MB_ALLOC(bad, 16);
-    MB_ALLOC(recs, nn * sizeof(DevPoint));
-    MB_ALLOC(sorted, nn * sizeof(DevPoint));
     cudaMemsetAsync(bad, 0, 16, s);
     cudaMemsetAsync(nruns, 0, 16, s);
     uint32_t h_runs = 0;
@@ -199,7 +185,8 @@ int map_build_device(MapDevHost& mh, const Globals& g, const float* d_xyz_world,
         cub::DeviceRunLengthEncode::Encode(nullptr, b2, keys_sorted, ukeys, counts, nruns, (int)n, s);
         cub::DeviceScan::ExclusiveSum(nullptr, b3, counts, starts, (int)n, s);
         tmp_bytes = std::max(b1, std::max(b2, b3));
-        MB_ALLOC(tmp, std::max<size_t>(tmp_bytes, 16));
+        LK_CUDA(err, b_tmp.alloc(std::max<size_t>(tmp_bytes, 16)));
+        void* tmp = b_tmp.p;
         // LSD radix sort is stable: equal keys keep ascending original index = insertion order
         cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, keys, keys_sorted, idx, idx_sorted, (int)n, 0, 63, s);
         cub::DeviceRunLengthEncode::Encode(tmp, tmp_bytes, keys_sorted, ukeys, counts, nruns, (int)n, s);
@@ -208,8 +195,8 @@ int map_build_device(MapDevHost& mh, const Globals& g, const float* d_xyz_world,
         cudaMemcpyAsync(&h_runs, nruns, 4, cudaMemcpyDeviceToHost, s);
         cudaMemcpyAsync(&h_bad, bad, 4, cudaMemcpyDeviceToHost, s);
         e = cudaStreamSynchronize(s);
-        if (e != cudaSuccess) { cleanup(); err = cudaGetErrorString(e); cudaGetLastError(); return LK_ERR_CUDA; }
-        if (h_bad) { cleanup(); err = "point outside the addressable key range (|key| >= 2^20)"; return LK_ERR_INVALID_ARG; }
+        if (e != cudaSuccess) { err = cudaGetErrorString(e); cudaGetLastError(); return LK_ERR_CUDA; }
+        if (h_bad) { err = "point outside the addressable key range (|key| >= 2^20)"; return LK_ERR_INVALID_ARG; }
         cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, counts, starts, (int)h_runs, s);
     }
     // size the map for this build plus the caller's reserve, then run the per-root warps;
@@ -242,7 +229,6 @@ int map_build_device(MapDevHost& mh, const Globals& g, const float* d_xyz_world,
         rc = LK_ERR_CAPACITY;
         err = "map pools overflowed repeatedly";
     }
-    cleanup();
     return rc;
 }
 

@@ -4,6 +4,7 @@
 #include <string>
 
 #include "lk_device.cuh"
+#include "lk_host.h"
 
 namespace lk {
 
@@ -12,13 +13,14 @@ struct MapDev;
 
 class MapDevHost {
    public:
-    ~MapDevHost() { release(); }
-    // (Re)create an EMPTY map sized for at least these counts plus the reserve; clears the table.
+    // (Re)create an EMPTY map sized for at least these counts plus the reserve; clears the table. On failure the handle
+    // holds no map (ready() is false, nothing allocated).
     int allocate(uint64_t roots, uint64_t nodes, uint64_t points, cudaStream_t s, std::string& err);
-    // Make sure pools can take `extra_*` more items (grows by reallocation + copy). No-op if they fit.
+    // Make sure pools can take `extra_*` more items (grows by reallocation + copy). No-op if they fit. On failure the
+    // existing pools are left as they were.
     int ensure_headroom(uint64_t extra_roots, uint64_t extra_nodes, uint64_t extra_points, cudaStream_t s,
                         std::string& err);
-    void release();
+    void release();  // drop the map (the reserve and the tile size stay)
     MapDev dev() const;
     bool ready() const { return hash_cap != 0; }
     // pull the device allocator counters (free lists included) into the host mirrors
@@ -30,14 +32,12 @@ class MapDevHost {
     uint64_t free_entries(int l) const;
     uint64_t pool_bytes() const;
 
-    HashSlot* slots = nullptr;
-    MapNode* nodes = nullptr;
-    MapAux* aux = nullptr;
-    HotRec* hot = nullptr;  // hot image of every node's plane (what the throughput kernel gathers)
-    DevPoint* points = nullptr;
-    // [0] n_nodes [1] n_roots [2] overflow [4..5] n_points (u64) [8] scratch [10..13] map_count_planes
+    // HashSlot[hash_cap] | MapNode, MapAux, HotRec[node_cap] (hot: the plane image the throughput kernel gathers) |
+    // DevPoint[point_cap]
+    DevBuf slots, nodes, aux, hot, points;
+    // uint32_t: [0] n_nodes [1] n_roots [2] overflow [4..5] n_points (u64) [8] scratch [10..13] map_count_planes
     // [16 + 3 l .. 18 + 3 l] avail | base | top of free list l (MapDev::free_ctr)
-    uint32_t* counters = nullptr;
+    DevBuf counters;
     uint64_t hash_cap = 0, node_cap = 0, point_cap = 0;
     uint32_t n_roots = 0, n_nodes = 0;
     uint64_t n_points = 0;  // bump pointer (slots handed out), not the number of live points
@@ -45,7 +45,7 @@ class MapDevHost {
     uint32_t tile_slots = 52;  // the standard point tile, even_up(max_points_num + 2) (set with the map config)
     // free lists: twice as many entries as the pool holds tiles / groups / nodes, so a launch that pops and then frees
     // every object again still finds room for the pending entries
-    uint32_t* free_items[3] = {nullptr, nullptr, nullptr};
+    DevBuf free_items[3];  // uint32_t
     uint64_t free_cap[3] = {0, 0, 0};
     int32_t free_avail[3] = {0, 0, 0};
     uint32_t free_base[3] = {0, 0, 0}, free_top[3] = {0, 0, 0};

@@ -97,31 +97,18 @@ uint64_t next_pow2(uint64_t v) {
     return p;
 }
 
-#define MI_CUDA(expr)                                                                          \
-    do {                                                                                       \
-        cudaError_t e__ = (expr);                                                              \
-        if (e__ != cudaSuccess) {                                                              \
-            cudaGetLastError();                                                                \
-            err = std::string(#expr) + ": " + cudaGetErrorString(e__);                         \
-            return e__ == cudaErrorMemoryAllocation ? LK_ERR_OUT_OF_MEMORY : LK_ERR_CUDA;      \
-        }                                                                                      \
-    } while (0)
-
 }  // namespace
 
 constexpr size_t COUNTER_BYTES = 128;
 constexpr int FREE_CTR = 16;  // first counter word of the free lists
 
 void MapDevHost::release() {
-    void* ptrs[] = {slots, nodes, aux, hot, points, counters, free_items[0], free_items[1], free_items[2]};
-    for (void* p : ptrs)
-        if (p) cudaFree(p);
-    slots = nullptr; nodes = nullptr; aux = nullptr; hot = nullptr; points = nullptr; counters = nullptr;
+    for (DevBuf* b : {&slots, &nodes, &aux, &hot, &points, &counters}) b->reset();
     hash_cap = node_cap = point_cap = 0;
     n_roots = n_nodes = 0;
     n_points = 0;
     for (int l = 0; l < 3; ++l) {
-        free_items[l] = nullptr;
+        free_items[l].reset();
         free_cap[l] = 0;
         free_avail[l] = 0; free_base[l] = free_top[l] = 0;
     }
@@ -135,13 +122,12 @@ int MapDevHost::size_free_lists(bool keep, cudaStream_t s, std::string& err) {
     for (int l = 0; l < 3; ++l) {
         if (!keep) { free_avail[l] = 0; free_base[l] = free_top[l] = 0; }
         if (want[l] <= free_cap[l]) continue;
-        uint32_t* p = nullptr;
-        MI_CUDA(cudaMalloc((void**)&p, want[l] * sizeof(uint32_t)));
+        DevBuf p;
+        LK_CUDA(err, p.alloc(want[l] * sizeof(uint32_t)));
         const uint64_t used = keep ? std::min<uint64_t>(free_top[l], free_cap[l]) : 0;
-        if (used) MI_CUDA(cudaMemcpyAsync(p, free_items[l], used * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
-        MI_CUDA(cudaStreamSynchronize(s));
-        if (free_items[l]) cudaFree(free_items[l]);
-        free_items[l] = p;
+        if (used) LK_CUDA(err, cudaMemcpyAsync(p.p, free_items[l].p, used * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
+        LK_CUDA(err, cudaStreamSynchronize(s));
+        free_items[l] = std::move(p);
         free_cap[l] = want[l];
     }
     return LK_OK;
@@ -153,68 +139,74 @@ uint64_t MapDevHost::free_entries(int l) const {
 
 uint64_t MapDevHost::pool_bytes() const {
     uint64_t b = hash_cap * sizeof(HashSlot) + node_cap * (sizeof(MapNode) + sizeof(MapAux) + sizeof(HotRec)) +
-                 point_cap * sizeof(DevPoint) + (counters ? COUNTER_BYTES : 0);
+                 point_cap * sizeof(DevPoint) + (counters.p ? COUNTER_BYTES : 0);
     for (int l = 0; l < 3; ++l) b += free_cap[l] * sizeof(uint32_t);
     return b;
 }
 
 MapDev MapDevHost::dev() const {
     MapDev d;
-    d.slots = slots;
+    uint32_t* ctr = counters.as<uint32_t>();
+    d.slots = slots.as<HashSlot>();
     d.hash_mask = (uint32_t)(hash_cap - 1);
-    d.nodes = nodes;
-    d.aux = aux;
-    d.hot = hot;
-    d.points = points;
+    d.nodes = nodes.as<MapNode>();
+    d.aux = aux.as<MapAux>();
+    d.hot = hot.as<HotRec>();
+    d.points = points.as<DevPoint>();
     d.node_cap = (uint32_t)node_cap;
     d.point_cap = point_cap;
-    d.n_nodes = counters;
-    d.n_roots = counters + 1;
-    d.overflow = counters + 2;
-    d.n_points = reinterpret_cast<unsigned long long*>(counters + 4);
+    d.n_nodes = ctr;
+    d.n_roots = ctr + 1;
+    d.overflow = ctr + 2;
+    d.n_points = reinterpret_cast<unsigned long long*>(ctr + 4);
     for (int l = 0; l < 3; ++l) {
-        d.free_items[l] = free_items[l];
+        d.free_items[l] = free_items[l].as<uint32_t>();
         d.free_cap[l] = (uint32_t)std::min<uint64_t>(free_cap[l], 0xffffffffu);
     }
-    d.free_ctr = counters ? counters + FREE_CTR : nullptr;
+    d.free_ctr = ctr ? ctr + FREE_CTR : nullptr;
     return d;
 }
 
 int MapDevHost::allocate(uint64_t roots, uint64_t nnodes, uint64_t npoints, cudaStream_t s, std::string& err) {
-    uint64_t want_hash = next_pow2(std::max<uint64_t>(1024, 4 * (roots + reserve_roots)));  // load factor <= 0.25
-    if (want_hash > (1ull << 31)) { err = "root table too large"; return LK_ERR_CAPACITY; }
-    uint64_t want_nodes = std::max<uint64_t>(nnodes + reserve_nodes, 64);
-    uint64_t want_points = std::max<uint64_t>(npoints + reserve_points, 64);
-    if (want_nodes >= (1ull << 31)) { err = "node pool too large"; return LK_ERR_CAPACITY; }
-    if (want_points >= (1ull << 32)) { err = "point pool too large"; return LK_ERR_CAPACITY; }
-    if (!counters) MI_CUDA(cudaMalloc((void**)&counters, COUNTER_BYTES));
-    if (want_hash != hash_cap) {
-        if (slots) cudaFree(slots);
-        slots = nullptr; hash_cap = 0;
-        MI_CUDA(cudaMalloc((void**)&slots, want_hash * sizeof(HashSlot)));
-        hash_cap = want_hash;
+    // Pools that are large enough are kept; a pool that is not is freed before its replacement is allocated. Any
+    // failure drops the whole map, so no caller goes ahead on a half-built one.
+    auto build = [&]() -> int {
+        uint64_t want_hash = next_pow2(std::max<uint64_t>(1024, 4 * (roots + reserve_roots)));  // load factor <= 0.25
+        if (want_hash > (1ull << 31)) { err = "root table too large"; return LK_ERR_CAPACITY; }
+        uint64_t want_nodes = std::max<uint64_t>(nnodes + reserve_nodes, 64);
+        uint64_t want_points = std::max<uint64_t>(npoints + reserve_points, 64);
+        if (want_nodes >= (1ull << 31)) { err = "node pool too large"; return LK_ERR_CAPACITY; }
+        if (want_points >= (1ull << 32)) { err = "point pool too large"; return LK_ERR_CAPACITY; }
+        if (!counters.p) LK_CUDA(err, counters.alloc(COUNTER_BYTES));
+        if (want_hash != hash_cap) {
+            hash_cap = 0;
+            LK_CUDA(err, slots.alloc(want_hash * sizeof(HashSlot)));
+            hash_cap = want_hash;
+        }
+        if (want_nodes > node_cap) {
+            nodes.reset(); aux.reset(); hot.reset(); node_cap = 0;
+            LK_CUDA(err, nodes.alloc(want_nodes * sizeof(MapNode)));
+            LK_CUDA(err, aux.alloc(want_nodes * sizeof(MapAux)));
+            LK_CUDA(err, hot.alloc(want_nodes * sizeof(HotRec)));
+            node_cap = want_nodes;
+        }
+        if (want_points > point_cap) {
+            point_cap = 0;
+            LK_CUDA(err, points.alloc(want_points * sizeof(DevPoint)));
+            point_cap = want_points;
+        }
+        int rc = size_free_lists(false, s, err);  // a new map starts with empty free lists
+        if (rc) return rc;
+        k_hash_clear<<<(unsigned)((hash_cap + 255) / 256), 256, 0, s>>>(slots.as<HashSlot>(), hash_cap);
+        LK_CUDA(err, cudaMemsetAsync(counters.p, 0, COUNTER_BYTES, s));
+        LK_CUDA(err, cudaGetLastError());
+        return LK_OK;
+    };
+    const int rc = build();
+    if (rc) {
+        release();
+        return rc;
     }
-    if (want_nodes > node_cap) {
-        if (nodes) cudaFree(nodes);
-        if (aux) cudaFree(aux);
-        if (hot) cudaFree(hot);
-        nodes = nullptr; aux = nullptr; hot = nullptr; node_cap = 0;
-        MI_CUDA(cudaMalloc((void**)&nodes, want_nodes * sizeof(MapNode)));
-        MI_CUDA(cudaMalloc((void**)&aux, want_nodes * sizeof(MapAux)));
-        MI_CUDA(cudaMalloc((void**)&hot, want_nodes * sizeof(HotRec)));
-        node_cap = want_nodes;
-    }
-    if (want_points > point_cap) {
-        if (points) cudaFree(points);
-        points = nullptr; point_cap = 0;
-        MI_CUDA(cudaMalloc((void**)&points, want_points * sizeof(DevPoint)));
-        point_cap = want_points;
-    }
-    int rc = size_free_lists(false, s, err);  // a new map starts with empty free lists
-    if (rc) return rc;
-    k_hash_clear<<<(unsigned)((hash_cap + 255) / 256), 256, 0, s>>>(slots, hash_cap);
-    MI_CUDA(cudaMemsetAsync(counters, 0, COUNTER_BYTES, s));
-    MI_CUDA(cudaGetLastError());
     n_roots = n_nodes = 0;
     n_points = 0;
     reallocs = 0;
@@ -228,29 +220,25 @@ int MapDevHost::ensure_headroom(uint64_t extra_roots, uint64_t extra_nodes, uint
     if (n_nodes + extra_nodes > node_cap) {
         uint64_t want = std::max<uint64_t>(n_nodes + extra_nodes, node_cap + node_cap / 2);
         if (want >= (1ull << 31)) { err = "node pool too large"; return LK_ERR_CAPACITY; }
-        MapNode* nn = nullptr;
-        MapAux* na = nullptr;
-        HotRec* nh = nullptr;
-        MI_CUDA(cudaMalloc((void**)&nn, want * sizeof(MapNode)));
-        MI_CUDA(cudaMalloc((void**)&na, want * sizeof(MapAux)));
-        MI_CUDA(cudaMalloc((void**)&nh, want * sizeof(HotRec)));
-        MI_CUDA(cudaMemcpyAsync(nn, nodes, (size_t)n_nodes * sizeof(MapNode), cudaMemcpyDeviceToDevice, s));
-        MI_CUDA(cudaMemcpyAsync(na, aux, (size_t)n_nodes * sizeof(MapAux), cudaMemcpyDeviceToDevice, s));
-        MI_CUDA(cudaMemcpyAsync(nh, hot, (size_t)n_nodes * sizeof(HotRec), cudaMemcpyDeviceToDevice, s));
-        MI_CUDA(cudaStreamSynchronize(s));
-        cudaFree(nodes); cudaFree(aux); cudaFree(hot);
-        nodes = nn; aux = na; hot = nh; node_cap = want;
+        DevBuf nn, na, nh;
+        LK_CUDA(err, nn.alloc(want * sizeof(MapNode)));
+        LK_CUDA(err, na.alloc(want * sizeof(MapAux)));
+        LK_CUDA(err, nh.alloc(want * sizeof(HotRec)));
+        LK_CUDA(err, cudaMemcpyAsync(nn.p, nodes.p, (size_t)n_nodes * sizeof(MapNode), cudaMemcpyDeviceToDevice, s));
+        LK_CUDA(err, cudaMemcpyAsync(na.p, aux.p, (size_t)n_nodes * sizeof(MapAux), cudaMemcpyDeviceToDevice, s));
+        LK_CUDA(err, cudaMemcpyAsync(nh.p, hot.p, (size_t)n_nodes * sizeof(HotRec), cudaMemcpyDeviceToDevice, s));
+        LK_CUDA(err, cudaStreamSynchronize(s));
+        nodes = std::move(nn); aux = std::move(na); hot = std::move(nh); node_cap = want;
         ++reallocs;
     }
     if (n_points + extra_points > point_cap) {
         uint64_t want = std::max<uint64_t>(n_points + extra_points, point_cap + point_cap / 2);
         if (want >= (1ull << 32)) { err = "point pool too large"; return LK_ERR_CAPACITY; }
-        DevPoint* np = nullptr;
-        MI_CUDA(cudaMalloc((void**)&np, want * sizeof(DevPoint)));
-        MI_CUDA(cudaMemcpyAsync(np, points, (size_t)n_points * sizeof(DevPoint), cudaMemcpyDeviceToDevice, s));
-        MI_CUDA(cudaStreamSynchronize(s));
-        cudaFree(points);
-        points = np; point_cap = want;
+        DevBuf np;
+        LK_CUDA(err, np.alloc(want * sizeof(DevPoint)));
+        LK_CUDA(err, cudaMemcpyAsync(np.p, points.p, (size_t)n_points * sizeof(DevPoint), cudaMemcpyDeviceToDevice, s));
+        LK_CUDA(err, cudaStreamSynchronize(s));
+        points = std::move(np); point_cap = want;
         ++reallocs;
     }
     int rc = size_free_lists(true, s, err);
@@ -259,18 +247,18 @@ int MapDevHost::ensure_headroom(uint64_t extra_roots, uint64_t extra_nodes, uint
         // rehash: dump roots, rebuild a bigger table
         uint64_t want = next_pow2(4 * (n_roots + extra_roots) + 4 * reserve_roots);
         if (want > (1ull << 31)) { err = "root table too large"; return LK_ERR_CAPACITY; }
-        lk_map_root* tmp = nullptr;
-        MI_CUDA(cudaMalloc((void**)&tmp, std::max<size_t>(n_roots, 1) * sizeof(lk_map_root)));
-        uint32_t* cnt = counters + 8;
-        MI_CUDA(cudaMemsetAsync(cnt, 0, 4, s));
-        k_hash_dump<<<(unsigned)((hash_cap + 255) / 256), 256, 0, s>>>(slots, hash_cap, tmp, cnt);
-        HashSlot* ns = nullptr;
-        MI_CUDA(cudaMalloc((void**)&ns, want * sizeof(HashSlot)));
-        k_hash_clear<<<(unsigned)((want + 255) / 256), 256, 0, s>>>(ns, want);
-        if (n_roots) k_hash_insert_roots<<<(n_roots + 255) / 256, 256, 0, s>>>(ns, (uint32_t)(want - 1), tmp, n_roots, counters + 2);
-        MI_CUDA(cudaStreamSynchronize(s));
-        cudaFree(slots); cudaFree(tmp);
-        slots = ns; hash_cap = want;
+        DevBuf tmp, ns;
+        LK_CUDA(err, tmp.alloc(std::max<size_t>(n_roots, 1) * sizeof(lk_map_root)));
+        uint32_t* cnt = counters.as<uint32_t>() + 8;
+        LK_CUDA(err, cudaMemsetAsync(cnt, 0, 4, s));
+        k_hash_dump<<<(unsigned)((hash_cap + 255) / 256), 256, 0, s>>>(slots.as<HashSlot>(), hash_cap, tmp.as<lk_map_root>(), cnt);
+        LK_CUDA(err, ns.alloc(want * sizeof(HashSlot)));
+        k_hash_clear<<<(unsigned)((want + 255) / 256), 256, 0, s>>>(ns.as<HashSlot>(), want);
+        if (n_roots)
+            k_hash_insert_roots<<<(n_roots + 255) / 256, 256, 0, s>>>(ns.as<HashSlot>(), (uint32_t)(want - 1), tmp.as<lk_map_root>(),
+                                                                     n_roots, counters.as<uint32_t>() + 2);
+        LK_CUDA(err, cudaStreamSynchronize(s));
+        slots = std::move(ns); hash_cap = want;
         ++reallocs;
     }
     return LK_OK;
@@ -278,8 +266,8 @@ int MapDevHost::ensure_headroom(uint64_t extra_roots, uint64_t extra_nodes, uint
 
 int MapDevHost::sync_counters(cudaStream_t s, std::string& err) {
     uint32_t h[FREE_CTR + 9] = {};
-    MI_CUDA(cudaMemcpyAsync(h, counters, sizeof(h), cudaMemcpyDeviceToHost, s));
-    MI_CUDA(cudaStreamSynchronize(s));
+    LK_CUDA(err, cudaMemcpyAsync(h, counters.p, sizeof(h), cudaMemcpyDeviceToHost, s));
+    LK_CUDA(err, cudaStreamSynchronize(s));
     n_nodes = h[0];
     n_roots = h[1];
     unsigned long long np;
@@ -301,7 +289,8 @@ int MapDevHost::push_counters(cudaStream_t s, std::string& err) {
         const uint32_t b = free_base[l];
         const uint32_t t = (uint32_t)std::min<uint64_t>(free_top[l], free_cap[l]);
         const uint32_t pend = t - b, k = std::min(b - a, pend);
-        if (k) MI_CUDA(cudaMemcpyAsync(free_items[l] + a, free_items[l] + (t - k), (size_t)k * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
+        uint32_t* items = free_items[l].as<uint32_t>();
+        if (k) LK_CUDA(err, cudaMemcpyAsync(items + a, items + (t - k), (size_t)k * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
         free_avail[l] = (int32_t)(a + pend);
         free_base[l] = free_top[l] = a + pend;
     }
@@ -313,8 +302,8 @@ int MapDevHost::push_counters(cudaStream_t s, std::string& err) {
         h[FREE_CTR + 3 * l + 1] = free_base[l];
         h[FREE_CTR + 3 * l + 2] = free_top[l];
     }
-    MI_CUDA(cudaMemcpyAsync(counters, h, sizeof(h), cudaMemcpyHostToDevice, s));
-    MI_CUDA(cudaStreamSynchronize(s));
+    LK_CUDA(err, cudaMemcpyAsync(counters.p, h, sizeof(h), cudaMemcpyHostToDevice, s));
+    LK_CUDA(err, cudaStreamSynchronize(s));
     return LK_OK;
 }
 
@@ -376,24 +365,24 @@ int map_upload_blob(MapDevHost& mh, const Globals& g, const void* blob, size_t b
     }
     int rc = mh.allocate(hd.n_roots, hd.n_nodes, slots_needed, s, err);
     if (rc) return rc;
-    lk_map_root* d_roots = nullptr;
-    MI_CUDA(cudaMalloc((void**)&d_roots, std::max<size_t>(hd.n_roots, 1) * sizeof(lk_map_root)));
+    DevBuf d_roots;
+    LK_CUDA(err, d_roots.alloc(std::max<size_t>(hd.n_roots, 1) * sizeof(lk_map_root)));
+    const MapDev md = mh.dev();
     cudaError_t e = cudaSuccess;
     if (hd.n_nodes) {
-        e = cudaMemcpyAsync(mh.nodes, nodes, (size_t)hd.n_nodes * sizeof(MapNode), cudaMemcpyHostToDevice, s);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(mh.aux, aux2.data(), (size_t)hd.n_nodes * sizeof(MapAux), cudaMemcpyHostToDevice, s);
+        e = cudaMemcpyAsync(md.nodes, nodes, (size_t)hd.n_nodes * sizeof(MapNode), cudaMemcpyHostToDevice, s);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(md.aux, aux2.data(), (size_t)hd.n_nodes * sizeof(MapAux), cudaMemcpyHostToDevice, s);
     }
-    if (e == cudaSuccess && !dpts.empty()) e = cudaMemcpyAsync(mh.points, dpts.data(), dpts.size() * sizeof(DevPoint), cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess && !dpts.empty()) e = cudaMemcpyAsync(md.points, dpts.data(), dpts.size() * sizeof(DevPoint), cudaMemcpyHostToDevice, s);
     if (e == cudaSuccess && hd.n_roots) {
-        e = cudaMemcpyAsync(d_roots, roots, (size_t)hd.n_roots * sizeof(lk_map_root), cudaMemcpyHostToDevice, s);
-        k_hash_insert_roots<<<(hd.n_roots + 255) / 256, 256, 0, s>>>(mh.slots, (uint32_t)(mh.hash_cap - 1), d_roots, hd.n_roots, mh.counters + 2);
-        k_check_roots<<<(hd.n_roots + 255) / 256, 256, 0, s>>>(mh.slots, (uint32_t)(mh.hash_cap - 1), d_roots, hd.n_roots, mh.counters + 2);
+        e = cudaMemcpyAsync(d_roots.p, roots, (size_t)hd.n_roots * sizeof(lk_map_root), cudaMemcpyHostToDevice, s);
+        k_hash_insert_roots<<<(hd.n_roots + 255) / 256, 256, 0, s>>>(md.slots, md.hash_mask, d_roots.as<lk_map_root>(), hd.n_roots, md.overflow);
+        k_check_roots<<<(hd.n_roots + 255) / 256, 256, 0, s>>>(md.slots, md.hash_mask, d_roots.as<lk_map_root>(), hd.n_roots, md.overflow);
     }
-    if (e == cudaSuccess && hd.n_nodes) k_hot_from_nodes<<<(hd.n_nodes + 255) / 256, 256, 0, s>>>(mh.nodes, mh.hot, hd.n_nodes);
+    if (e == cudaSuccess && hd.n_nodes) k_hot_from_nodes<<<(hd.n_nodes + 255) / 256, 256, 0, s>>>(md.nodes, md.hot, hd.n_nodes);
     uint32_t ovf = 0;
-    if (e == cudaSuccess) e = cudaMemcpyAsync(&ovf, mh.counters + 2, 4, cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&ovf, md.overflow, 4, cudaMemcpyDeviceToHost, s);
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    cudaFree(d_roots);
     if (e != cudaSuccess) { cudaGetLastError(); err = cudaGetErrorString(e); return LK_ERR_CUDA; }
     if (ovf & 8u) { err = "duplicate root keys in the blob"; return LK_ERR_BAD_BLOB; }
     if (ovf) { err = "root table overflow"; return LK_ERR_CAPACITY; }
@@ -418,8 +407,8 @@ int map_download_blob(MapDevHost& mh, void* blob, size_t capacity, size_t* bytes
     int rc = mh.sync_counters(s, err);
     if (rc) return rc;
     std::vector<lk_map_aux> aux(mh.n_nodes);
-    if (mh.n_nodes) MI_CUDA(cudaMemcpyAsync(aux.data(), mh.aux, (size_t)mh.n_nodes * sizeof(MapAux), cudaMemcpyDeviceToHost, s));
-    MI_CUDA(cudaStreamSynchronize(s));
+    if (mh.n_nodes) LK_CUDA(err, cudaMemcpyAsync(aux.data(), mh.aux.p, (size_t)mh.n_nodes * sizeof(MapAux), cudaMemcpyDeviceToHost, s));
+    LK_CUDA(err, cudaStreamSynchronize(s));
     uint64_t live = 0;
     for (auto& a : aux) live += (uint64_t)std::max(a.pts_count, 0);
     size_t need = sizeof(lk_map_blob_header) + (size_t)mh.n_roots * sizeof(lk_map_root) +
@@ -434,22 +423,21 @@ int map_download_blob(MapDevHost& mh, void* blob, size_t capacity, size_t* bytes
     char* p = (char*)blob;
     std::memcpy(p, &hd, sizeof(hd));
     p += sizeof(hd);
-    lk_map_root* d_roots = nullptr;
-    MI_CUDA(cudaMalloc((void**)&d_roots, std::max<size_t>(mh.n_roots, 1) * sizeof(lk_map_root)));
-    uint32_t* cnt = mh.counters + 8;
+    DevBuf d_roots;
+    LK_CUDA(err, d_roots.alloc(std::max<size_t>(mh.n_roots, 1) * sizeof(lk_map_root)));
+    uint32_t* cnt = mh.counters.as<uint32_t>() + 8;
     cudaMemsetAsync(cnt, 0, 4, s);
-    k_hash_dump<<<(unsigned)((mh.hash_cap + 255) / 256), 256, 0, s>>>(mh.slots, mh.hash_cap, d_roots, cnt);
-    cudaError_t e = cudaMemcpyAsync(p, d_roots, (size_t)mh.n_roots * sizeof(lk_map_root), cudaMemcpyDeviceToHost, s);
+    k_hash_dump<<<(unsigned)((mh.hash_cap + 255) / 256), 256, 0, s>>>(mh.slots.as<HashSlot>(), mh.hash_cap, d_roots.as<lk_map_root>(), cnt);
+    cudaError_t e = cudaMemcpyAsync(p, d_roots.p, (size_t)mh.n_roots * sizeof(lk_map_root), cudaMemcpyDeviceToHost, s);
     p += (size_t)mh.n_roots * sizeof(lk_map_root);
-    if (e == cudaSuccess && mh.n_nodes) e = cudaMemcpyAsync(p, mh.nodes, (size_t)mh.n_nodes * sizeof(MapNode), cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess && mh.n_nodes) e = cudaMemcpyAsync(p, mh.nodes.p, (size_t)mh.n_nodes * sizeof(MapNode), cudaMemcpyDeviceToHost, s);
     p += (size_t)mh.n_nodes * sizeof(MapNode);
     lk_map_aux* out_aux = (lk_map_aux*)p;
     p += (size_t)mh.n_nodes * sizeof(MapAux);
     lk_map_point* out_pts = (lk_map_point*)p;
     std::vector<DevPoint> dpts((size_t)mh.n_points);
-    if (e == cudaSuccess && mh.n_points) e = cudaMemcpyAsync(dpts.data(), mh.points, (size_t)mh.n_points * sizeof(DevPoint), cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess && mh.n_points) e = cudaMemcpyAsync(dpts.data(), mh.points.p, (size_t)mh.n_points * sizeof(DevPoint), cudaMemcpyDeviceToHost, s);
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    cudaFree(d_roots);
     if (e != cudaSuccess) { cudaGetLastError(); err = cudaGetErrorString(e); return LK_ERR_CUDA; }
     uint64_t at = 0;
     for (uint32_t i = 0; i < mh.n_nodes; ++i) {
@@ -473,18 +461,19 @@ int map_clear_outside(MapDevHost& mh, const int lo[3], const int hi[3], uint64_t
     int rc = mh.sync_counters(s, err);
     if (rc) return rc;
     if (mh.n_roots == 0) return LK_OK;
-    lk_map_root* d_roots = nullptr;
-    uint32_t* d_cnt = nullptr;
-    MI_CUDA(cudaMalloc((void**)&d_roots, (size_t)mh.n_roots * sizeof(lk_map_root)));
-    MI_CUDA(cudaMalloc((void**)&d_cnt, 4));
-    MI_CUDA(cudaMemsetAsync(d_cnt, 0, 4, s));
-    k_hash_dump<<<(unsigned)((mh.hash_cap + 255) / 256), 256, 0, s>>>(mh.slots, mh.hash_cap, d_roots, d_cnt);
+    DevBuf d_roots, d_cnt;
+    LK_CUDA(err, d_roots.alloc((size_t)mh.n_roots * sizeof(lk_map_root)));
+    LK_CUDA(err, d_cnt.alloc(4));
+    LK_CUDA(err, cudaMemsetAsync(d_cnt.p, 0, 4, s));
+    const MapDev md = mh.dev();
+    lk_map_root* dr = d_roots.as<lk_map_root>();
+    k_hash_dump<<<(unsigned)((mh.hash_cap + 255) / 256), 256, 0, s>>>(md.slots, mh.hash_cap, dr, d_cnt.as<uint32_t>());
     std::vector<lk_map_root> roots(mh.n_roots);
     uint32_t n = 0;
-    cudaError_t e = cudaMemcpyAsync(&n, d_cnt, 4, cudaMemcpyDeviceToHost, s);
+    cudaError_t e = cudaMemcpyAsync(&n, d_cnt.p, 4, cudaMemcpyDeviceToHost, s);
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    if (e == cudaSuccess && n) e = cudaMemcpy(roots.data(), d_roots, (size_t)std::min(n, mh.n_roots) * sizeof(lk_map_root), cudaMemcpyDeviceToHost);
-    if (e != cudaSuccess) { cudaFree(d_roots); cudaFree(d_cnt); cudaGetLastError(); err = cudaGetErrorString(e); return LK_ERR_CUDA; }
+    if (e == cudaSuccess && n) e = cudaMemcpy(roots.data(), dr, (size_t)std::min(n, mh.n_roots) * sizeof(lk_map_root), cudaMemcpyDeviceToHost);
+    if (e != cudaSuccess) { cudaGetLastError(); err = cudaGetErrorString(e); return LK_ERR_CUDA; }
     n = std::min(n, mh.n_roots);
     // kept roots first, dropped ones after them
     std::vector<lk_map_root> gone;
@@ -498,14 +487,13 @@ int map_clear_outside(MapDevHost& mh, const int lo[3], const int hi[3], uint64_t
     if (removed) *removed = n - keep;
     if (keep != n) {
         std::copy(gone.begin(), gone.end(), roots.begin() + keep);
-        e = cudaMemcpyAsync(d_roots, roots.data(), (size_t)n * sizeof(lk_map_root), cudaMemcpyHostToDevice, s);
-        k_hash_clear<<<(unsigned)((mh.hash_cap + 255) / 256), 256, 0, s>>>(mh.slots, mh.hash_cap);
-        if (keep) k_hash_insert_roots<<<(keep + 255) / 256, 256, 0, s>>>(mh.slots, (uint32_t)(mh.hash_cap - 1), d_roots, keep, mh.counters + 2);
+        e = cudaMemcpyAsync(dr, roots.data(), (size_t)n * sizeof(lk_map_root), cudaMemcpyHostToDevice, s);
+        k_hash_clear<<<(unsigned)((mh.hash_cap + 255) / 256), 256, 0, s>>>(md.slots, mh.hash_cap);
+        if (keep) k_hash_insert_roots<<<(keep + 255) / 256, 256, 0, s>>>(md.slots, md.hash_mask, dr, keep, md.overflow);
         // their storage is recycled by the next launch that grows the map
-        k_free_subtrees<<<(n - keep + 127) / 128, 128, 0, s>>>(mh.dev(), d_roots + keep, n - keep, (int)mh.tile_slots);
+        k_free_subtrees<<<(n - keep + 127) / 128, 128, 0, s>>>(md, dr + keep, n - keep, (int)mh.tile_slots);
         if (e == cudaSuccess) e = cudaStreamSynchronize(s);
     }
-    cudaFree(d_roots); cudaFree(d_cnt);
     if (e != cudaSuccess) { cudaGetLastError(); err = cudaGetErrorString(e); return LK_ERR_CUDA; }
     if (keep == n) return LK_OK;
     rc = mh.sync_counters(s, err);  // the free lists as the kernel left them
@@ -520,12 +508,12 @@ int map_count_planes(MapDevHost& mh, uint64_t* planes, uint64_t* live_points, cu
     if (!mh.ready()) return LK_OK;
     int rc = mh.sync_counters(s, err);
     if (rc) return rc;
-    unsigned long long* out = reinterpret_cast<unsigned long long*>(mh.counters + 10);
-    MI_CUDA(cudaMemsetAsync(out, 0, 16, s));
-    if (mh.n_nodes) k_count_planes<<<(mh.n_nodes + 255) / 256, 256, 0, s>>>(mh.nodes, mh.aux, mh.n_nodes, out);
+    unsigned long long* out = reinterpret_cast<unsigned long long*>(mh.counters.as<uint32_t>() + 10);
+    LK_CUDA(err, cudaMemsetAsync(out, 0, 16, s));
+    if (mh.n_nodes) k_count_planes<<<(mh.n_nodes + 255) / 256, 256, 0, s>>>(mh.nodes.as<MapNode>(), mh.aux.as<MapAux>(), mh.n_nodes, out);
     unsigned long long h[2] = {0, 0};
-    MI_CUDA(cudaMemcpyAsync(h, out, 16, cudaMemcpyDeviceToHost, s));
-    MI_CUDA(cudaStreamSynchronize(s));
+    LK_CUDA(err, cudaMemcpyAsync(h, out, 16, cudaMemcpyDeviceToHost, s));
+    LK_CUDA(err, cudaStreamSynchronize(s));
     *planes = h[0];
     *live_points = h[1];
     return LK_OK;

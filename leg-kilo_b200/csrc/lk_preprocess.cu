@@ -13,6 +13,7 @@
 #include <string>
 
 #include "lk_device.cuh"
+#include "lk_host.h"
 
 namespace lk {
 
@@ -150,58 +151,41 @@ __global__ void k_bucket_heads(const float4* __restrict__ pts, const uint32_t* _
     curv[pos[i]] = pts[i].w;
 }
 
-struct Tmp {
-    void* p = nullptr;
-    ~Tmp() { if (p) cudaFree(p); }
-    cudaError_t get(size_t b) { return cudaMalloc(&p, b ? b : 16); }
-    template <class T> T* as() { return reinterpret_cast<T*>(p); }
-};
-
 }  // namespace
-
-#define PP_CUDA(expr)                                                            \
-    do {                                                                         \
-        cudaError_t e__ = (expr);                                                \
-        if (e__ != cudaSuccess) {                                                \
-            cudaGetLastError();                                                  \
-            err = std::string(#expr) + ": " + cudaGetErrorString(e__);           \
-            return e__ == cudaErrorMemoryAllocation ? LK_ERR_OUT_OF_MEMORY : LK_ERR_CUDA; \
-        }                                                                        \
-    } while (0)
 
 int decode_pointcloud2_device(const uint8_t* h_data, uint32_t n, const lk_pc2_layout& L, float blind, int filter_num,
                               double time_scale, float* h_pts_out, float* h_intensity_out, uint32_t* n_out, cudaStream_t s,
                               std::string& err) {
     *n_out = 0;
     if (!n) return LK_OK;
-    Tmp d_data, d_flags, d_pos, d_out, d_int, d_tmp;
+    DevBuf d_data, d_flags, d_pos, d_out, d_int, d_tmp;
     const size_t bytes = (size_t)n * L.point_step;
-    PP_CUDA(d_data.get(bytes));
-    PP_CUDA(d_flags.get((size_t)n * 4));
-    PP_CUDA(d_pos.get((size_t)n * 4));
-    PP_CUDA(d_out.get((size_t)n * 16));
-    PP_CUDA(d_int.get((size_t)n * 4));
-    PP_CUDA(cudaMemcpyAsync(d_data.p, h_data, bytes, cudaMemcpyHostToDevice, s));
+    LK_CUDA(err, d_data.alloc(bytes));
+    LK_CUDA(err, d_flags.alloc((size_t)n * 4));
+    LK_CUDA(err, d_pos.alloc((size_t)n * 4));
+    LK_CUDA(err, d_out.alloc((size_t)n * 16));
+    LK_CUDA(err, d_int.alloc((size_t)n * 4));
+    LK_CUDA(err, cudaMemcpyAsync(d_data.p, h_data, bytes, cudaMemcpyHostToDevice, s));
     const unsigned g = (n + 255) / 256;
     k_decode_flags<<<g, 256, 0, s>>>(d_data.as<uint8_t>(), n, L, blind, filter_num, d_flags.as<uint32_t>());
     size_t tb = 0;
     cub::DeviceScan::ExclusiveSum(nullptr, tb, d_flags.as<uint32_t>(), d_pos.as<uint32_t>(), (int)n, s);
-    PP_CUDA(d_tmp.get(tb));
+    LK_CUDA(err, d_tmp.alloc(tb));
     cub::DeviceScan::ExclusiveSum(d_tmp.p, tb, d_flags.as<uint32_t>(), d_pos.as<uint32_t>(), (int)n, s);
     k_decode_scatter<<<g, 256, 0, s>>>(d_data.as<uint8_t>(), n, L, time_scale, d_flags.as<uint32_t>(), d_pos.as<uint32_t>(),
                                        d_out.as<float4>(), h_intensity_out ? d_int.as<float>() : nullptr);
     uint32_t last_pos = 0, last_flag = 0;
-    PP_CUDA(cudaMemcpyAsync(&last_pos, d_pos.as<uint32_t>() + (n - 1), 4, cudaMemcpyDeviceToHost, s));
-    PP_CUDA(cudaMemcpyAsync(&last_flag, d_flags.as<uint32_t>() + (n - 1), 4, cudaMemcpyDeviceToHost, s));
-    PP_CUDA(cudaStreamSynchronize(s));
+    LK_CUDA(err, cudaMemcpyAsync(&last_pos, d_pos.as<uint32_t>() + (n - 1), 4, cudaMemcpyDeviceToHost, s));
+    LK_CUDA(err, cudaMemcpyAsync(&last_flag, d_flags.as<uint32_t>() + (n - 1), 4, cudaMemcpyDeviceToHost, s));
+    LK_CUDA(err, cudaStreamSynchronize(s));
     const uint32_t m = last_pos + last_flag;
     *n_out = m;
     if (m) {
-        PP_CUDA(cudaMemcpyAsync(h_pts_out, d_out.p, (size_t)m * 16, cudaMemcpyDeviceToHost, s));
-        if (h_intensity_out) PP_CUDA(cudaMemcpyAsync(h_intensity_out, d_int.p, (size_t)m * 4, cudaMemcpyDeviceToHost, s));
-        PP_CUDA(cudaStreamSynchronize(s));
+        LK_CUDA(err, cudaMemcpyAsync(h_pts_out, d_out.p, (size_t)m * 16, cudaMemcpyDeviceToHost, s));
+        if (h_intensity_out) LK_CUDA(err, cudaMemcpyAsync(h_intensity_out, d_int.p, (size_t)m * 4, cudaMemcpyDeviceToHost, s));
+        LK_CUDA(err, cudaStreamSynchronize(s));
     }
-    PP_CUDA(cudaGetLastError());
+    LK_CUDA(err, cudaGetLastError());
     return LK_OK;
 }
 
@@ -211,17 +195,17 @@ int preprocess_scan_device(const float* h_pts_in, uint32_t n, float leaf, float*
     *n_out = 0;
     *n_buckets = 0;
     if (!n) { h_bucket_offsets[0] = 0; return LK_OK; }
-    Tmp d_in, d_mm, d_idx, d_ord, d_idx2, d_ord2, d_uk, d_cnt, d_st, d_nr, d_cent, d_cb, d_lid, d_cb2, d_lid2, d_out, d_heads,
+    DevBuf d_in, d_mm, d_idx, d_ord, d_idx2, d_ord2, d_uk, d_cnt, d_st, d_nr, d_cent, d_cb, d_lid, d_cb2, d_lid2, d_out, d_heads,
         d_pos, d_off, d_curv, d_tmp;
-    PP_CUDA(d_in.get((size_t)n * 16));
-    PP_CUDA(d_mm.get(64));
-    PP_CUDA(cudaMemcpyAsync(d_in.p, h_pts_in, (size_t)n * 16, cudaMemcpyHostToDevice, s));
+    LK_CUDA(err, d_in.alloc((size_t)n * 16));
+    LK_CUDA(err, d_mm.alloc(64));
+    LK_CUDA(err, cudaMemcpyAsync(d_in.p, h_pts_in, (size_t)n * 16, cudaMemcpyHostToDevice, s));
     int mm0[6] = {INT_MAX, INT_MAX, INT_MAX, INT_MIN, INT_MIN, INT_MIN};
-    PP_CUDA(cudaMemcpyAsync(d_mm.p, mm0, sizeof(mm0), cudaMemcpyHostToDevice, s));
+    LK_CUDA(err, cudaMemcpyAsync(d_mm.p, mm0, sizeof(mm0), cudaMemcpyHostToDevice, s));
     k_minmax<<<std::min<unsigned>((n + 255) / 256, 1184u), 256, 0, s>>>(d_in.as<float4>(), n, d_mm.as<int>());
     int mm[6];
-    PP_CUDA(cudaMemcpyAsync(mm, d_mm.p, sizeof(mm), cudaMemcpyDeviceToHost, s));
-    PP_CUDA(cudaStreamSynchronize(s));
+    LK_CUDA(err, cudaMemcpyAsync(mm, d_mm.p, sizeof(mm), cudaMemcpyDeviceToHost, s));
+    LK_CUDA(err, cudaStreamSynchronize(s));
     auto ord2f_h = [](int i) { int j = i >= 0 ? i : i ^ 0x7fffffff; float f; std::memcpy(&f, &j, 4); return f; };
     GridParams gp;
     gp.inv_leaf = 1.0f / leaf;  // inverse_leaf_size_ = Ones / leaf_size_ (float)
@@ -238,66 +222,66 @@ int preprocess_scan_device(const float* h_pts_in, uint32_t n, float leaf, float*
     }
     gp.mul[0] = 1; gp.mul[1] = div_b[0]; gp.mul[2] = div_b[0] * div_b[1];
     const unsigned g = (n + 255) / 256;
-    PP_CUDA(d_idx.get((size_t)n * 4)); PP_CUDA(d_ord.get((size_t)n * 4)); PP_CUDA(d_idx2.get((size_t)n * 4)); PP_CUDA(d_ord2.get((size_t)n * 4));
-    PP_CUDA(d_uk.get((size_t)n * 4)); PP_CUDA(d_cnt.get((size_t)n * 4)); PP_CUDA(d_st.get((size_t)n * 4)); PP_CUDA(d_nr.get(16));
+    LK_CUDA(err, d_idx.alloc((size_t)n * 4)); LK_CUDA(err, d_ord.alloc((size_t)n * 4)); LK_CUDA(err, d_idx2.alloc((size_t)n * 4)); LK_CUDA(err, d_ord2.alloc((size_t)n * 4));
+    LK_CUDA(err, d_uk.alloc((size_t)n * 4)); LK_CUDA(err, d_cnt.alloc((size_t)n * 4)); LK_CUDA(err, d_st.alloc((size_t)n * 4)); LK_CUDA(err, d_nr.alloc(16));
     k_leaf_index<<<g, 256, 0, s>>>(d_in.as<float4>(), n, gp, d_idx.as<uint32_t>(), d_ord.as<uint32_t>());
     size_t b1 = 0, b2 = 0, b3 = 0;
     cub::DeviceRadixSort::SortPairs(nullptr, b1, d_idx.as<uint32_t>(), d_idx2.as<uint32_t>(), d_ord.as<uint32_t>(), d_ord2.as<uint32_t>(), (int)n, 0, 32, s);
     cub::DeviceRunLengthEncode::Encode(nullptr, b2, d_idx2.as<uint32_t>(), d_uk.as<uint32_t>(), d_cnt.as<uint32_t>(), d_nr.as<uint32_t>(), (int)n, s);
     cub::DeviceScan::ExclusiveSum(nullptr, b3, d_cnt.as<uint32_t>(), d_st.as<uint32_t>(), (int)n, s);
     const size_t tb = std::max(b1, std::max(b2, b3));
-    PP_CUDA(d_tmp.get(tb));
+    LK_CUDA(err, d_tmp.alloc(tb));
     size_t tb2 = tb;
     cub::DeviceRadixSort::SortPairs(d_tmp.p, tb2, d_idx.as<uint32_t>(), d_idx2.as<uint32_t>(), d_ord.as<uint32_t>(), d_ord2.as<uint32_t>(), (int)n, 0, 32, s);
     tb2 = tb;
     cub::DeviceRunLengthEncode::Encode(d_tmp.p, tb2, d_idx2.as<uint32_t>(), d_uk.as<uint32_t>(), d_cnt.as<uint32_t>(), d_nr.as<uint32_t>(), (int)n, s);
     uint32_t n_leaves = 0;
-    PP_CUDA(cudaMemcpyAsync(&n_leaves, d_nr.p, 4, cudaMemcpyDeviceToHost, s));
-    PP_CUDA(cudaStreamSynchronize(s));
+    LK_CUDA(err, cudaMemcpyAsync(&n_leaves, d_nr.p, 4, cudaMemcpyDeviceToHost, s));
+    LK_CUDA(err, cudaStreamSynchronize(s));
     tb2 = tb;
     cub::DeviceScan::ExclusiveSum(d_tmp.p, tb2, d_cnt.as<uint32_t>(), d_st.as<uint32_t>(), (int)n_leaves, s);
-    PP_CUDA(d_cent.get((size_t)n_leaves * 16)); PP_CUDA(d_cb.get((size_t)n_leaves * 4)); PP_CUDA(d_lid.get((size_t)n_leaves * 4));
-    PP_CUDA(d_cb2.get((size_t)n_leaves * 4)); PP_CUDA(d_lid2.get((size_t)n_leaves * 4)); PP_CUDA(d_out.get((size_t)n_leaves * 16));
-    PP_CUDA(d_heads.get((size_t)n_leaves * 4)); PP_CUDA(d_pos.get((size_t)n_leaves * 4));
-    PP_CUDA(d_off.get(((size_t)n_leaves + 1) * 4)); PP_CUDA(d_curv.get((size_t)n_leaves * 4));
-    PP_CUDA(cudaMemsetAsync(d_nr.p, 0, 16, s));
+    LK_CUDA(err, d_cent.alloc((size_t)n_leaves * 16)); LK_CUDA(err, d_cb.alloc((size_t)n_leaves * 4)); LK_CUDA(err, d_lid.alloc((size_t)n_leaves * 4));
+    LK_CUDA(err, d_cb2.alloc((size_t)n_leaves * 4)); LK_CUDA(err, d_lid2.alloc((size_t)n_leaves * 4)); LK_CUDA(err, d_out.alloc((size_t)n_leaves * 16));
+    LK_CUDA(err, d_heads.alloc((size_t)n_leaves * 4)); LK_CUDA(err, d_pos.alloc((size_t)n_leaves * 4));
+    LK_CUDA(err, d_off.alloc(((size_t)n_leaves + 1) * 4)); LK_CUDA(err, d_curv.alloc((size_t)n_leaves * 4));
+    LK_CUDA(err, cudaMemsetAsync(d_nr.p, 0, 16, s));
     k_centroids<<<(n_leaves + 127) / 128, 128, 0, s>>>(d_in.as<float4>(), d_ord2.as<uint32_t>(), d_uk.as<uint32_t>(), d_cnt.as<uint32_t>(),
                                                        d_st.as<uint32_t>(), n_leaves, d_cent.as<float4>(), d_cb.as<uint32_t>(),
                                                        d_lid.as<uint32_t>(), d_nr.as<uint32_t>());
     uint32_t n_valid = 0;
-    PP_CUDA(cudaMemcpyAsync(&n_valid, d_nr.p, 4, cudaMemcpyDeviceToHost, s));
-    PP_CUDA(cudaStreamSynchronize(s));
+    LK_CUDA(err, cudaMemcpyAsync(&n_valid, d_nr.p, 4, cudaMemcpyDeviceToHost, s));
+    LK_CUDA(err, cudaStreamSynchronize(s));
     // non-finite points form the LAST run (key 0xffffffff) and were skipped: the first n_valid leaves are the output
     if (n_valid) {
         size_t c1 = 0;
         cub::DeviceRadixSort::SortPairs(nullptr, c1, d_cb.as<uint32_t>(), d_cb2.as<uint32_t>(), d_lid.as<uint32_t>(), d_lid2.as<uint32_t>(), (int)n_valid, 0, 32, s);
-        Tmp d_t2;
-        PP_CUDA(d_t2.get(c1));
+        DevBuf d_t2;
+        LK_CUDA(err, d_t2.alloc(c1));
         cub::DeviceRadixSort::SortPairs(d_t2.p, c1, d_cb.as<uint32_t>(), d_cb2.as<uint32_t>(), d_lid.as<uint32_t>(), d_lid2.as<uint32_t>(), (int)n_valid, 0, 32, s);
         const unsigned gl = (n_valid + 255) / 256;
         k_gather_sorted<<<gl, 256, 0, s>>>(d_cent.as<float4>(), d_lid2.as<uint32_t>(), n_valid, d_out.as<float4>(), d_heads.as<uint32_t>());
         size_t c2 = 0;
         cub::DeviceScan::ExclusiveSum(nullptr, c2, d_heads.as<uint32_t>(), d_pos.as<uint32_t>(), (int)n_valid, s);
-        Tmp d_t3;
-        PP_CUDA(d_t3.get(c2));
+        DevBuf d_t3;
+        LK_CUDA(err, d_t3.alloc(c2));
         cub::DeviceScan::ExclusiveSum(d_t3.p, c2, d_heads.as<uint32_t>(), d_pos.as<uint32_t>(), (int)n_valid, s);
         k_bucket_heads<<<gl, 256, 0, s>>>(d_out.as<float4>(), d_heads.as<uint32_t>(), d_pos.as<uint32_t>(), n_valid, d_off.as<uint32_t>(), d_curv.as<float>());
         uint32_t lp = 0, lh = 0;
-        PP_CUDA(cudaMemcpyAsync(&lp, d_pos.as<uint32_t>() + (n_valid - 1), 4, cudaMemcpyDeviceToHost, s));
-        PP_CUDA(cudaMemcpyAsync(&lh, d_heads.as<uint32_t>() + (n_valid - 1), 4, cudaMemcpyDeviceToHost, s));
-        PP_CUDA(cudaStreamSynchronize(s));
+        LK_CUDA(err, cudaMemcpyAsync(&lp, d_pos.as<uint32_t>() + (n_valid - 1), 4, cudaMemcpyDeviceToHost, s));
+        LK_CUDA(err, cudaMemcpyAsync(&lh, d_heads.as<uint32_t>() + (n_valid - 1), 4, cudaMemcpyDeviceToHost, s));
+        LK_CUDA(err, cudaStreamSynchronize(s));
         const uint32_t nb = lp + lh;
-        PP_CUDA(cudaMemcpyAsync(h_pts_out, d_out.p, (size_t)n_valid * 16, cudaMemcpyDeviceToHost, s));
-        PP_CUDA(cudaMemcpyAsync(h_bucket_offsets, d_off.p, (size_t)nb * 4, cudaMemcpyDeviceToHost, s));
-        PP_CUDA(cudaMemcpyAsync(h_bucket_curv, d_curv.p, (size_t)nb * 4, cudaMemcpyDeviceToHost, s));
-        PP_CUDA(cudaStreamSynchronize(s));
+        LK_CUDA(err, cudaMemcpyAsync(h_pts_out, d_out.p, (size_t)n_valid * 16, cudaMemcpyDeviceToHost, s));
+        LK_CUDA(err, cudaMemcpyAsync(h_bucket_offsets, d_off.p, (size_t)nb * 4, cudaMemcpyDeviceToHost, s));
+        LK_CUDA(err, cudaMemcpyAsync(h_bucket_curv, d_curv.p, (size_t)nb * 4, cudaMemcpyDeviceToHost, s));
+        LK_CUDA(err, cudaStreamSynchronize(s));
         h_bucket_offsets[nb] = n_valid;
         *n_buckets = nb;
     } else {
         h_bucket_offsets[0] = 0;
     }
     *n_out = n_valid;
-    PP_CUDA(cudaGetLastError());
+    LK_CUDA(err, cudaGetLastError());
     return LK_OK;
 }
 
