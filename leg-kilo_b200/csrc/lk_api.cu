@@ -836,6 +836,7 @@ static FusedArgs fused_args(lk_handle h, uint32_t first, int iters, bool insert,
     fa.mv.slots = md.slots;
     fa.mv.hash_mask = md.hash_mask;
     fa.mv.nodes = md.nodes;
+    fa.mv.hot = md.hot;
     if (mq) {
         fa.imu = mq->d_imu;
         fa.kin = mq->d_kin;
@@ -957,7 +958,7 @@ static int run_kernels(lk_handle h, uint32_t first, uint32_t count, int iters, b
                 launch_scan_tail(ra, first, count, s);
                 if (c1 > c0) h->acc_launches += 2;
             } else {
-                launch_residual(ra, c1 - c0, false, s);
+                launch_residual(ra, c1 - c0, false, !update_map, s);
             }
             if (timed) cudaEventRecord(kev_get(h, h->nev++), s);
             if (c1 > c0) { ++h->acc_launches; ++h->acc_residual_launches; }
@@ -1175,7 +1176,7 @@ int lk_debug_residuals(lk_handle h, const lk_state* x, const double* P, const fl
     ra.dbg_z = h->dbg_z.as<double>();
     ra.dbg_R = h->dbg_R.as<double>();
     ra.dbg_key = h->dbg_key.as<int32_t>();
-    launch_residual(ra, h->total_chunks, true, s);
+    launch_residual(ra, h->total_chunks, true, true, s);
     LK_CUDA(h->err, cudaGetLastError());
     if (n) {
         if (ok_out) LK_CUDA(h->err, cudaMemcpyAsync(ok_out, h->dbg_ok.p, n, cudaMemcpyDeviceToHost, s));

@@ -45,6 +45,8 @@ __device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src_gmem, u
                  : "memory");
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// the same between this thread's view of global memory and the bulk copies it issues next
+__device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
 
 __device__ __forceinline__ void mbar_init_fence() {
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");

@@ -67,7 +67,8 @@ __host__ __device__ inline void hot_from_node(const lk_map_node& nd, HotRec& h) 
 struct MapView {  // what the residual path reads of the map
     const HashSlot* slots;
     uint32_t hash_mask;
-    const MapNode* nodes;
+    const MapNode* nodes;  // full records: the octree descent below a root that holds no plane
+    const HotRec* hot;     // plane images of the nodes: what the per-point passes gather
 };
 
 // ---- per-call constants (kernel parameter space) ------------------------------------------

@@ -54,20 +54,23 @@ struct PredictScratch {
     ObsScratch obs;  // the IMU / Kin+IMU update follows its predict, so both live here
 };
 
-struct FusedSmem {
+// HOT: the passes stage hot plane images (a map that stays fixed for the launch), else node records (lk_pass.cuh: Stage)
+template <bool HOT>
+struct FusedSmemT {
     BlockFilter f;
     ScanConst sc;
     double slice[WARPS * 32];
     double clk[2];
     union {  // predict and the point passes never overlap in time
         PredictScratch pr;
-        PassSmem<BLOCK> pass;
+        PassSmem<BLOCK, HOT> pass;
     } u;
 };
+typedef FusedSmemT<true> FusedSmem;  // without the map insert
 
 // with the map insert inside: the plane-fit staging tiles of the warps, with their own mbarriers (initialised once)
 struct FusedSmemIns {
-    FusedSmem base;
+    FusedSmemT<false> base;  // the map changes between buckets: node records
     WarpTile wt[WARPS];
     MapDev md;   // copies for the out-of-line insert phase
     Globals g;
@@ -84,12 +87,32 @@ __device__ __noinline__ void fused_insert_phase2(FusedSmemIns* si, const uint32_
         warp_insert_root_scan(md, si->g, wt, __ldcg(&touched[t]), iroot, ipts, n_bucket, pend, lane);
 }
 
-static_assert(sizeof(PredictScratch) <= sizeof(((PassSmem<BLOCK>*)0)->tile), "predict scratch must not reach the mbarriers");
+static_assert(sizeof(PredictScratch) <= sizeof(((PassSmem<BLOCK, true>*)0)->tile) &&
+                  sizeof(PredictScratch) <= sizeof(((PassSmem<BLOCK, false>*)0)->tile),
+              "predict scratch must not reach the mbarriers");
 static_assert(sizeof(FusedSmemIns) <= 227 * 1024, "one block per SM");
+// The block's shared memory plus the 1 KiB the driver reserves per block must fit the 132 KiB carve-out: the remaining
+// 124 KiB of L1 then hold the stack frames of all 256 threads (a few hundred bytes each) beside the cached point and table
+// reads, so their spill traffic stays in L1. With the node-record tiles (the map-insert variant) it needs 164 KiB or more.
+static_assert(sizeof(FusedSmem) + 1024 <= 132 * 1024, "the batch-of-one kernel's stack frames must fit in L1");
+
+// The smallest shared-memory carve-out that holds one block of `smem` bytes, as the percentage
+// cudaFuncAttributePreferredSharedMemoryCarveout takes (the driver rounds up to the next carve-out the SM supports). Without
+// it the driver may pick a larger carve-out than one block needs, and the L1 left for the stack frames shrinks.
+int carveout_percent(size_t smem, int dev) {
+    int per_sm = 0, per_block = 0;
+    cudaDeviceGetAttribute(&per_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev);
+    cudaDeviceGetAttribute(&per_block, cudaDevAttrReservedSharedMemoryPerBlock, dev);
+    if (per_sm <= 0) return 100;
+    const size_t need = smem + (size_t)per_block;
+    const int pct = (int)((need * 100 + (size_t)per_sm - 1) / (size_t)per_sm);
+    return pct < 100 ? pct : 100;
+}
 
 // KILO.cc:110-115: covariance with dt since the last UPDATE, state with dt since the last PREDICT; F is built
 // from the pre-propagation state. Out of line: a scan-at-once call (bucket time == both clocks) never gets here.
-__device__ __noinline__ void fused_predict(FusedSmem* sm, const double* Q, double dtc, double dt) {
+template <class SM>
+__device__ __noinline__ void fused_predict(SM* sm, const double* Q, double dtc, double dt) {
     if (dtc != 0.0) {
         build_F(sm->u.pr.F, sm->f.x, dtc);
         cov_predict(sm->f.P, sm->u.pr.F, sm->u.pr.T, sm->u.pr.Ps, Q, dtc);
@@ -104,7 +127,8 @@ __device__ __noinline__ void fused_predict(FusedSmem* sm, const double* Q, doubl
 }
 
 // every queued inertial / kinematic sample older than this bucket (KILO.cc:379-390)
-__device__ __noinline__ void fused_drain_queue(FusedSmem* sm, const FusedArgs& a, uint32_t& mi, double t_bucket) {
+template <class SM>
+__device__ __noinline__ void fused_drain_queue(SM* sm, const FusedArgs& a, uint32_t& mi, double t_bucket) {
     bool drained = false;
     while (mi < a.n_meas) {
         const double ts = a.imu ? a.imu[mi].stamp : a.kin[mi].stamp;
@@ -130,6 +154,8 @@ template <> struct InlineSel<false> { typedef FusedNoInline type; };
 // fences its earlier global writes. Acquire side: a gpu-scope fence AFTER the barrier — on this architecture it also
 // invalidates the SM's L1 (CCTL.IVALL, see the SASS), so the plain (L1-cached) loads of the next phase cannot be served from
 // a line cached before another SM rewrote it; the read-only path (ld.global.nc) is not used on the map in these kernels.
+// The next bucket's pass reads the node records the insert just wrote with generic stores through bulk copies (async
+// proxy): a proxy fence after the acquire orders the two.
 __device__ __forceinline__ void grid_sync(const FusedArgs& a, uint32_t& sync_idx) {
     __threadfence();
     __syncthreads();
@@ -137,6 +163,7 @@ __device__ __forceinline__ void grid_sync(const FusedArgs& a, uint32_t& sync_idx
     ++sync_idx;
     __syncthreads();
     __threadfence();
+    fence_proxy_async_global();
 }
 
 // OBS: an inertial / kinematic queue is drained before every bucket. INL: the small inputs ride in the parameter block.
@@ -145,7 +172,7 @@ template <bool OBS, bool INL, bool INS>
 __global__ void __launch_bounds__(BLOCK, 1) k_scan_fused(const __grid_constant__ FusedArgs a,
                                                          const __grid_constant__ typename InlineSel<INL>::type inl) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    FusedSmem* sm = reinterpret_cast<FusedSmem*>(smem_raw);
+    FusedSmemT<!INS>* sm = reinterpret_cast<FusedSmemT<!INS>*>(smem_raw);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const uint32_t scan = a.scan;
     // let the next launch of the stream (if it was launched with programmatic serialisation) start placing its
@@ -179,7 +206,7 @@ __global__ void __launch_bounds__(BLOCK, 1) k_scan_fused(const __grid_constant__
         if (tid == 0) si->md = a.md;
         if (tid < (int)(sizeof(Globals) / 4)) reinterpret_cast<uint32_t*>(&si->g)[tid] = reinterpret_cast<const uint32_t*>(&a.g)[tid];
     }
-    pass_init<BLOCK>(&sm->u.pass);  // mbarrier init fence + block barrier
+    pass_init(&sm->u.pass);  // mbarrier init fence + block barrier
     FT(1);
     uint32_t n_eff_total = 0;
     uint32_t phase = 0;
@@ -329,6 +356,8 @@ cudaError_t launch_one(const FusedArgs& a, const FusedInline* inl, uint32_t grid
     cudaGetDevice(&dev);
     if (dev >= 0 && dev < 64 && !attr[dev]) {
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM);
+        if (e != cudaSuccess) return e;
+        e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, carveout_percent(SMEM, dev));
         if (e != cudaSuccess) return e;
         attr[dev] = true;
     }

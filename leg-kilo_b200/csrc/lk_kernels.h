@@ -51,8 +51,9 @@ struct ResidualArgs {
 constexpr uint32_t S2_FB_WARPS = 6, S2_FB_CAP = 704;
 
 // Every chunk of the launch holds at most 256 points (one point per thread, one pass), except with debug
-// (lk_debug_residuals), where a block walks its chunk in 256-point slices and writes per-point rows
-void launch_residual(const ResidualArgs& a, uint32_t n_chunks, bool debug, cudaStream_t s);
+// (lk_debug_residuals), where a block walks its chunk in 256-point slices and writes per-point rows. hot: the map stays fixed
+// for the call, so the pass stages hot plane images instead of node records (lk_pass.cuh: Stage)
+void launch_residual(const ResidualArgs& a, uint32_t n_chunks, bool debug, bool hot, cudaStream_t s);
 // throughput family: pipelined residual pass (lk_stream2.cu) writing one partial row per chunk, then the per-scan
 // solve for scans [scan_first, scan_first + n_scans) (lk_residual.cu)
 void launch_residual_stream2(const ResidualArgs& a, uint32_t n_chunks, cudaStream_t s);

@@ -3,22 +3,40 @@
 // kernel and the debug rows (lk_residual.cu):
 //   1. transform, voxel key, home probe AND the speculative probe of the one neighbour voxel the
 //      reference falls back to (KILO.cc:156-178) — both 16-byte table reads are in flight together;
-//   2. every lane stages its 256-byte home and neighbour plane records into shared memory with TMA bulk
-//      copies (cp.async.bulk global -> shared, completion on the warp's mbarrier) instead of 15 scattered
-//      128-bit loads per lane and record (32 cache lines per warp-instruction);
-//   3. gates + residual row from the staged record (conflict-free 128-bit shared loads, 272-byte
-//      slot stride);
+//   2. every lane stages what it evaluates of its home and neighbour roots into shared memory with TMA bulk copies
+//      (cp.async.bulk global -> shared, completion on the warp's mbarrier) instead of scattered 128-bit loads:
+//      HOT = the 144-byte hot plane images (lk_device.cuh: HotRec), else the first 240 bytes of the node records;
+//   3. gates + residual row from the staged slot (conflict-free 128-bit shared loads); with HOT, a root that holds
+//      no plane reads its node record and descends into its children (eval_descent, rare);
 //   4. points whose home voxel gave no residual are compacted into a block-wide list and their
 //      neighbour record is evaluated by the first threads of the block — a few percent of the
 //      points fail, but almost every warp holds one, so without compaction every warp would pay
 //      the second round.
 #pragma once
+#include <cstddef>
+
 #include "lk_async.cuh"
 #include "lk_point.cuh"
 
 namespace lk {
 
-constexpr int TILE_STRIDE = 272;  // 256-byte record + 16: 128-bit reads of 8 consecutive lanes hit 32 banks
+// What a lane stages per root, and the slot stride of the tiles: an odd number of 16-byte units, so the 128-bit reads of 8
+// consecutive lanes fall into 8 disjoint groups of 4 banks.
+//   HOT = false: the 15 x 16 bytes of the node record plane_from_smem reads (centre .. flags / child_base), 240-byte slots.
+//   HOT = true: the 144 used bytes of the hot image (eval_plane_hot), 176-byte slots.
+// The hot image evaluates sigma_plane in the collapsed form a^T Scc a - 2 a^T v + s, which rounds differently from the
+// 21-term form of the node record (about 1e-16 relative). A pass over a map that stays fixed for the call takes the hot
+// images, like the throughput family; a call that updates the map takes the node records, so that the rounding does not
+// compound through the points it inserts (the map-vs-reference parity of the streaming path is bitwise in the form it has).
+template <bool HOT> struct Stage;
+template <> struct Stage<false> { static constexpr uint32_t BYTES = 240; static constexpr int STRIDE = 240; };
+template <> struct Stage<true> { static constexpr uint32_t BYTES = 144; static constexpr int STRIDE = 176; };
+static_assert(offsetof(lk_map_node, child_base) + sizeof(int32_t) <= Stage<false>::BYTES && Stage<false>::BYTES % 16 == 0 &&
+                  Stage<false>::STRIDE >= (int)Stage<false>::BYTES && Stage<false>::STRIDE % 32 == 16,
+              "staged record slots");
+static_assert(Stage<true>::BYTES % 16 == 0 && Stage<true>::BYTES <= sizeof(HotRec) && Stage<true>::STRIDE >= (int)Stage<true>::BYTES &&
+                  Stage<true>::STRIDE % 32 == 16,
+              "staged hot image slots");
 
 __device__ __forceinline__ void plane_from_smem(const unsigned char* slot, PlaneRec& r) {
     const double2* q = reinterpret_cast<const double2*>(slot);
@@ -160,6 +178,29 @@ __device__ __forceinline__ bool eval_record(const MapNode* __restrict__ nodes, c
     return false;
 }
 
+// One root through build_single_residual (voxel_map.cc:363-427) from its staged hot image: the plane decides, or, when
+// the root holds no plane, the descent into its children.
+template <bool COH = false>
+__device__ __forceinline__ bool eval_root(const MapNode* __restrict__ nodes, int root, const unsigned char* slot, const PointCtx& pc,
+                                          const ScanConst& sc, const Globals& g, Row& row) {
+    const int rc = eval_plane_hot(slot, pc, sc, g, row);
+    if (rc != 1) return rc == 0;
+    return eval_descent<COH>(nodes, root, pc, sc, g, row);
+}
+
+// One root from its staged slot, in the form HOT selects.
+template <bool COH, bool HOT>
+__device__ __forceinline__ bool eval_staged(const MapNode* __restrict__ nodes, int root, const unsigned char* slot, const PointCtx& pc,
+                                            const ScanConst& sc, const Globals& g, Row& row) {
+    if constexpr (HOT) {
+        return eval_root<COH>(nodes, root, slot, pc, sc, g, row);
+    } else {
+        PlaneRec r;
+        plane_from_smem(slot, r);
+        return eval_record<COH>(nodes, r, pc, sc, g, row);
+    }
+}
+
 // =================================================================================================
 // The block-wide pass. In the fused per-scan kernel a block keeps one chunk, so a lane sees the same point in every
 // iteration of a bucket: the lane keeps everything that does not depend on the state, plus the last voxel key with its
@@ -175,23 +216,24 @@ struct LaneCache {
     int have;  // 0 = nothing cached, 1 = point quantities cached, 2 = + keys / root / near / staged records
 };
 
-template <int NTHREADS>
+template <int NTHREADS, bool HOT>
 struct PassSmem {
-    __align__(16) unsigned char tile[2][NTHREADS * TILE_STRIDE];  // [0] home records, [1] neighbour records
+    static constexpr int STRIDE = Stage<HOT>::STRIDE;
+    __align__(16) unsigned char tile[2][NTHREADS * STRIDE];  // [0] home roots, [1] neighbour roots (Stage<HOT>)
     // Every lane's point context of the current pass. The evaluations read it from here and the descent receives its
     // address, so it never lives in the stack frame (which the L1 left beside this much shared memory cannot hold: every
     // access would go to L2); the fallback round reads the failing lane's context in place, without a copy.
     PointCtx pt[NTHREADS];
     struct __align__(8) Fallback {
-        int near;
-        uint32_t idx;  // the failing lane: its context is pt[idx], its neighbour record tile[1] slot idx
+        int near;      // the neighbour root (its node record, should a descent be needed)
+        uint32_t idx;  // the failing lane: its context is pt[idx], its neighbour's staged slot tile[1] slot idx
     } fb[NTHREADS];
     uint64_t bar[NTHREADS / 32];
     uint32_t wcnt[NTHREADS / 32];
 };
 
-template <int NTHREADS>
-__device__ __forceinline__ void pass_init(PassSmem<NTHREADS>* ps) {
+template <class PS>
+__device__ __forceinline__ void pass_init(PS* ps) {
     const int tid = threadIdx.x;
     if ((tid & 31) == 0) mbar_init(&ps->bar[tid >> 5], 1);
     mbar_init_fence();
@@ -201,8 +243,8 @@ __device__ __forceinline__ void pass_init(PassSmem<NTHREADS>* ps) {
 // `phase` is the warp's mbarrier parity (start at 0, carried between passes). Every row goes to sink(idx, row), `idx` being
 // the thread that holds the point: a thread passes its own home row, then the fallback row it evaluated for another
 // thread. Both calls follow both evaluations, so nothing the sink keeps (the accumulators) is live across an evaluation.
-template <int NTHREADS, bool COH = false, class Sink>
-__device__ __forceinline__ void points_pass(PassSmem<NTHREADS>* ps, uint32_t& phase, uint32_t count, const ScanConst& sc,
+template <int NTHREADS, bool COH = false, bool HOT, class Sink>
+__device__ __forceinline__ void points_pass(PassSmem<NTHREADS, HOT>* ps, uint32_t& phase, uint32_t count, const ScanConst& sc,
                                             const MapView& mv, const Globals& g, LaneCache& lc, float4 pre, Sink sink) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const bool active = (uint32_t)tid < count;
@@ -257,26 +299,27 @@ __device__ __forceinline__ void points_pass(PassSmem<NTHREADS>* ps, uint32_t& ph
         lc.root = root; lc.near = near;
         lc.have = 2;
     }
-    // ---- stage the records: one bulk copy per lane and record ---------------------------------------
-    unsigned char* home_slot = ps->tile[0] + (size_t)tid * TILE_STRIDE;
-    unsigned char* near_slot = ps->tile[1] + (size_t)tid * TILE_STRIDE;
+    // ---- stage the roots: one bulk copy per lane and root ---------------------------------------
+    constexpr uint32_t BYTES = Stage<HOT>::BYTES;
+    unsigned char* home_slot = ps->tile[0] + (size_t)tid * ps->STRIDE;
+    unsigned char* near_slot = ps->tile[1] + (size_t)tid * ps->STRIDE;
+    auto src = [&](int r) -> const void* {
+        if constexpr (HOT) return mv.hot + r;
+        else return mv.nodes + r;
+    };
     const uint32_t vh = __ballot_sync(0xffffffffu, gather_home), vn = __ballot_sync(0xffffffffu, gather_near);
     if (vh | vn) {
-        if (lane == 0) mbar_expect_tx(&ps->bar[warp], 256u * (uint32_t)(__popc(vh) + __popc(vn)));
+        if (lane == 0) mbar_expect_tx(&ps->bar[warp], BYTES * (uint32_t)(__popc(vh) + __popc(vn)));
         __syncwarp();
-        if (gather_home) bulk_g2s(home_slot, mv.nodes + root, 256u, &ps->bar[warp]);
-        if (gather_near) bulk_g2s(near_slot, mv.nodes + near, 256u, &ps->bar[warp]);
+        if (gather_home) bulk_g2s(home_slot, src(root), BYTES, &ps->bar[warp]);
+        if (gather_near) bulk_g2s(near_slot, src(near), BYTES, &ps->bar[warp]);
         mbar_wait(&ps->bar[warp], phase);
         phase ^= 1u;
     }
     // ---- gates + row -----------------------------------------------------------------------------
     Row row;
     bool ok = false;
-    if (root >= 0) {
-        PlaneRec r;
-        plane_from_smem(home_slot, r);
-        ok = eval_record<COH>(mv.nodes, r, pc, sc, g, row);
-    }
+    if (root >= 0) ok = eval_staged<COH, HOT>(mv.nodes, root, home_slot, pc, sc, g, row);
     {  // the failing points, listed per warp in lane order (no atomics: the order, hence the sums, are reproducible); entry
        // `tid` of the warp-major concatenation of the lists is handled by thread `tid`; their contexts stay in pt
         const bool want = root >= 0 && !ok && near >= 0;
@@ -289,15 +332,14 @@ __device__ __forceinline__ void points_pass(PassSmem<NTHREADS>* ps, uint32_t& ph
         }
     }
     __syncthreads();
-    // ---- fallback round: the neighbour voxel of the points that failed at home, record already staged -------
+    // ---- fallback round: the neighbour voxel of the points that failed at home, already staged -------
     uint32_t fb_slot = 0, idx = 0;
     Row row2;
     bool ok2 = false;
     if (fallback_pick<NTHREADS>(ps, fb_slot)) {
-        idx = ps->fb[fb_slot].idx;
-        PlaneRec r;
-        plane_from_smem(ps->tile[1] + (size_t)idx * TILE_STRIDE, r);
-        ok2 = eval_record<COH>(mv.nodes, r, ps->pt[idx], sc, g, row2);
+        const auto f = ps->fb[fb_slot];
+        idx = f.idx;
+        ok2 = eval_staged<COH, HOT>(mv.nodes, f.near, ps->tile[1] + (size_t)idx * ps->STRIDE, ps->pt[idx], sc, g, row2);
     }
     if (ok) sink((uint32_t)tid, row);
     if (ok2) sink(idx, row2);

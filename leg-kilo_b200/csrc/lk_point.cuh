@@ -121,6 +121,51 @@ __device__ __forceinline__ bool eval_plane(const PlaneRec& r, const PointCtx& pc
     return true;
 }
 
+// eval_plane (need_prob = false) on a staged hot image (lk_device.cuh: HotRec, 144 bytes, 16-byte aligned, nine 128-bit
+// loads): sigma_plane = a^T Scc a - 2 a^T v + s. Everything else as eval_plane.
+// Returns 0 = row produced, 1 = the node holds no plane (octree descent needed), 2 = a plane, but the point is gated out.
+__device__ __forceinline__ int eval_plane_hot(const unsigned char* slot, const PointCtx& pc, const ScanConst& sc, const Globals& g,
+                                              Row& row) {
+    const double2* q = reinterpret_cast<const double2*>(slot);
+    const float2 dr = *reinterpret_cast<const float2*>(q + 8);
+    if (dr.y < 0.0f) return 1;  // no plane in this node
+    const double2 v0 = q[0], v1 = q[1], v2 = q[2];
+    const double c0 = v0.x, c1 = v0.y, c2 = v1.x, n0 = v1.y, n1 = v2.x, n2 = v2.y;
+    const double s = n0 * pc.pwx + n1 * pc.pwy + n2 * pc.pwz + (double)dr.x;
+    const float dis = (float)fabs(s);
+    const double ax = pc.pwx - c0, ay = pc.pwy - c1, az = pc.pwz - c2;
+    const float dc = (float)(ax * ax + ay * ay + az * az);
+    const float rd = sqrtf(__fsub_rn(dc, __fmul_rn(dis, dis)));
+    if (!((double)rd <= 3.0 * (double)dr.y)) return 2;
+    const double2 v3 = q[3], v4 = q[4], v5 = q[5], v6 = q[6], v7 = q[7];
+    const double scc[6] = {v3.x, v3.y, v4.x, v4.y, v5.x, v5.y};
+    const double sigma_pl = quad_sym3(scc, ax, ay, az) - 2.0 * (ax * v6.x + ay * v6.y + az * v7.x) + v7.y;
+    const double qx = sc.R[0] * n0 + sc.R[3] * n1 + sc.R[6] * n2;
+    const double qy = sc.R[1] * n0 + sc.R[4] * n1 + sc.R[7] * n2;
+    const double qz = sc.R[2] * n0 + sc.R[5] * n1 + sc.R[8] * n2;
+    const double hx = pc.piy * qz - pc.piz * qy, hy = pc.piz * qx - pc.pix * qz, hz = pc.pix * qy - pc.piy * qx;
+    const double wx = g.Re[0] * qx + g.Re[3] * qy + g.Re[6] * qz;
+    const double wy = g.Re[1] * qx + g.Re[4] * qy + g.Re[7] * qz;
+    const double wz = g.Re[2] * qx + g.Re[5] * qy + g.Re[8] * qz;
+    const double uw = pc.pbx * wx + pc.pby * wy + pc.pbz * wz;
+    const double ww = wx * wx + wy * wy + wz * wz;
+    const double uw2 = uw * uw / pc.r2;
+    const double body = (double)g.rv * uw2 + pc.range2 * g.dv * (ww - uw2);
+    const double state = quad_sym3(sc.Pth, hx, hy, hz) + quad_sym3(sc.Ppp, n0, n1, n2);
+    const double sigma_l = sigma_pl + body + state;
+    const double lhs = (double)dis * (double)dis;
+    const double rhs = g.sigma_num * g.sigma_num * sigma_l;
+    bool pass;
+    if (lhs < rhs * (1.0 - 1e-12)) pass = true;
+    else if (lhs > rhs * (1.0 + 1e-12)) pass = false;
+    else pass = (double)dis < g.sigma_num * sqrt(sigma_l);
+    if (!pass) return 2;
+    row.h[0] = hx; row.h[1] = hy; row.h[2] = hz; row.h[3] = n0; row.h[4] = n1; row.h[5] = n2;
+    row.z = -(double)(float)s;
+    row.R = g.ratio * (sigma_pl + body);
+    return 0;
+}
+
 __device__ __forceinline__ int map_find(const HashSlot* __restrict__ slots, uint32_t mask, int kx, int ky, int kz) {
     uint32_t i = hash_key(kx, ky, kz) & mask;
     for (;;) {
@@ -171,6 +216,21 @@ static __device__ __noinline__ bool visit_subtree(const MapNode* __restrict__ no
     *probp = prob;
     *rowp = row;
     return ok;
+}
+
+// Root `root` holds no plane (eval_plane_hot returned 1): its flags and child base, one dependent read of the node record
+// (rare), then the descent into its children as build_single_residual does (voxel_map.cc:412-424).
+template <bool COH = false>
+__device__ __forceinline__ bool eval_descent(const MapNode* __restrict__ nodes, int root, const PointCtx& pc, const ScanConst& sc,
+                                             const Globals& g, Row& row) {
+    if (g.max_layer < 1) return false;
+    const uint2* fcp = reinterpret_cast<const uint2*>(&nodes[root].flags);
+    const uint2 fc = COH ? __ldcg(fcp) : __ldg(fcp);
+    const uint32_t cmask = (fc.x >> LK_NODE_CHILDMASK_SHIFT) & 0xffu;
+    const int child_base = (int)fc.y;
+    if (child_base < 0 || !cmask) return false;
+    double prob = 0.0;
+    return visit_subtree<COH>(nodes, child_base, cmask, &pc, &sc, &g, &prob, &row);
 }
 
 // One point through rows a3-a7. Returns true when a residual row was produced.

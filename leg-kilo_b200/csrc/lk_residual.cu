@@ -63,30 +63,32 @@ __device__ void scan_solve(const ResidualArgs& a, uint32_t scan, TailSmem* ts) {
     }
 }
 
+template <bool HOT>
 union ResidualSmem {  // the tail runs after the pass: same storage
-    PassSmem<BLOCK> pass;
+    PassSmem<BLOCK, HOT> pass;
     TailSmem tail;
 };
 
 // One pass over the block's chunk (at most BLOCK points on this path), its rows summed into the chunk's partial row; the last
 // block of a scan solves. DEBUG (lk_debug_residuals): the chunk may be longer, so the block walks it in BLOCK-point slices and
 // writes every point's row and voxel key instead of summing.
-template <bool DEBUG>
+// HOT: the pass stages hot plane images (a map that stays fixed for the call), else node records (lk_pass.cuh: Stage).
+template <bool DEBUG, bool HOT>
 __global__ void __launch_bounds__(BLOCK, 1) k_residual(const __grid_constant__ ResidualArgs a) {
     extern __shared__ __align__(16) unsigned char s_raw[];
     __shared__ ScanConst s_sc;
     __shared__ uint32_t s_last;
-    ResidualSmem* rs = reinterpret_cast<ResidualSmem*>(s_raw);
+    ResidualSmem<HOT>* rs = reinterpret_cast<ResidualSmem<HOT>*>(s_raw);
     TailSmem* ts = &rs->tail;
     const int tid = threadIdx.x;
     LK_TRACE(0);
     const ChunkDesc cd = a.chunks[a.chunk_first + blockIdx.x];
     if (tid < (int)(sizeof(ScanConst) / sizeof(double)))
         reinterpret_cast<double*>(&s_sc)[tid] = reinterpret_cast<const double*>(a.sc + cd.scan)[tid];
-    pass_init<BLOCK>(&rs->pass);
+    pass_init(&rs->pass);
     LK_TRACE(1);
     MapView mv;
-    mv.slots = a.slots; mv.hash_mask = a.hash_mask; mv.nodes = a.nodes;
+    mv.slots = a.slots; mv.hash_mask = a.hash_mask; mv.nodes = a.nodes; mv.hot = a.hot;
     double acc[32];
 #pragma unroll
     for (int i = 0; i < 32; ++i) acc[i] = 0.0;
@@ -177,18 +179,24 @@ void launch_scan_tail(const ResidualArgs& a, uint32_t scan_first, uint32_t n_sca
     k_scan_tail<<<n_scans, BLOCK, sizeof(TailSmem), s>>>(a, scan_first);
 }
 
-void launch_residual(const ResidualArgs& a, uint32_t n_chunks, bool debug, cudaStream_t s) {
-    if (n_chunks == 0) return;
+template <bool HOT>
+void launch_residual_as(const ResidualArgs& a, uint32_t n_chunks, bool debug, cudaStream_t s) {
     static PerDeviceOnce once;
-    const size_t smem = sizeof(ResidualSmem);
+    const size_t smem = sizeof(ResidualSmem<HOT>);
     if (once.first()) {
-        cudaFuncSetAttribute(k_residual<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        cudaFuncSetAttribute(k_residual<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        cudaFuncSetAttribute(k_residual<true, HOT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        cudaFuncSetAttribute(k_residual<false, HOT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     }
     if (debug)
-        k_residual<true><<<n_chunks, BLOCK, smem, s>>>(a);
+        k_residual<true, HOT><<<n_chunks, BLOCK, smem, s>>>(a);
     else
-        k_residual<false><<<n_chunks, BLOCK, smem, s>>>(a);
+        k_residual<false, HOT><<<n_chunks, BLOCK, smem, s>>>(a);
+}
+
+void launch_residual(const ResidualArgs& a, uint32_t n_chunks, bool debug, bool hot, cudaStream_t s) {
+    if (n_chunks == 0) return;
+    if (hot) launch_residual_as<true>(a, n_chunks, debug, s);
+    else launch_residual_as<false>(a, n_chunks, debug, s);
 }
 
 // ---- re-projection with the updated state (KILO.cc:216-224) ---------------------------------
