@@ -202,6 +202,8 @@ int lk_host_free(void* p);
  *   "fused_insert" 0 (default); 1 = a streaming scan (update_map) runs entirely inside ONE persistent kernel, the map
  *                 insert included (DESIGN.md 3.5; currently slower than the per-bucket kernels)
  *   "slim_p"      1 (default) blocks that never read the full covariance load only the strip they need (fused kernel)
+ *   "debug_records" 0 (default) lk_debug_residuals evaluates the hot plane images, as calls with a fixed map do;
+ *                 1 = the node records, as calls with update_map do (the two round sigma_plane differently)
  *   "kernel_timing", "trace": measurement / debugging aids
  * Any other name fails with LK_ERR_INVALID_ARG. */
 int lk_set_param(lk_handle h, const char* name, double value);

@@ -112,6 +112,7 @@ struct lk_context {
     int fast_insert = 1;  // update_map: two-launch insert for small buckets, re-projection folded into it
     int fused_insert = 0;  // 1 = update_map of one scan with small buckets: UpdateVoxelMap inside the persistent kernel (one
                            // launch per scan; the serial per-root insert chain holds every other SM at the grid barrier)
+    int debug_records = 0;  // 1 = lk_debug_residuals stages node records (the form update_map calls evaluate), not hot images
     bool direct = false, direct_ran = false, inline_ok = false;
     const float4* direct_pts = nullptr;
     float4* direct_world = nullptr;
@@ -414,7 +415,8 @@ int lk_set_param(lk_handle h, const char* name, double value) {
                  {"lane_cache", &lk_context::lane_cache},       {"fast_insert", &lk_context::fast_insert},
                  {"fused_insert", &lk_context::fused_insert},   {"coop_launch", &lk_context::coop_launch},
                  {"pdl", &lk_context::pdl},                     {"slim_p", &lk_context::slim_p},
-                 {"direct_io", &lk_context::direct_io},         {"inline_in", &lk_context::inline_in}};
+                 {"direct_io", &lk_context::direct_io},         {"inline_in", &lk_context::inline_in},
+                 {"debug_records", &lk_context::debug_records}};
     for (const auto& k : knobs)
         if (!std::strcmp(name, k.name)) {
             h->*k.knob = (int)value;
@@ -1176,7 +1178,7 @@ int lk_debug_residuals(lk_handle h, const lk_state* x, const double* P, const fl
     ra.dbg_z = h->dbg_z.as<double>();
     ra.dbg_R = h->dbg_R.as<double>();
     ra.dbg_key = h->dbg_key.as<int32_t>();
-    launch_residual(ra, h->total_chunks, true, true, s);
+    launch_residual(ra, h->total_chunks, true, !h->debug_records, s);
     LK_CUDA(h->err, cudaGetLastError());
     if (n) {
         if (ok_out) LK_CUDA(h->err, cudaMemcpyAsync(ok_out, h->dbg_ok.p, n, cudaMemcpyDeviceToHost, s));
