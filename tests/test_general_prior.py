@@ -1,0 +1,154 @@
+"""The CPU oracle at general priors: a first-frame map built from a rotated, off-origin pose, a prior composed from it, and
+a dense SPD P0 (optionally with a skew part) whose attitude / position blocks weigh in the gate. Pins the oracle's
+handling of P's row-major layout, its 3 x 3 blocks and its cross covariances to the reference, so that the device tests
+of tests/test_gpu_general_prior.py compare against a trusted oracle.
+
+- against tests/golden/ref_general_*.npz (tests/golden/make_ref_general_golden.py, made by the reference itself), in both
+  gain modes, with the tolerances of tests/test_reference_golden.py;
+- against the compiled reference on random general priors (any attitude, positions within +-3 km, random dense P0 with
+  or without a skew part, all four dataset configurations), where it is available."""
+import os
+
+import numpy as np
+import pytest
+
+import general_prior as gp
+import lko
+import lkref
+import mapcmp
+from legkilo_b200 import abi, synth
+
+GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+BUCKETS = ["leg_fusion", "hilti", "asym", "far"]
+
+
+def load(name):
+    d = dict(np.load(os.path.join(GOLD, name)))
+    for k in ("x0", "x"):
+        d[k] = d[k].view(abi.STATE_DTYPE)
+    for k in ("clk0", "clk"):
+        d[k] = d[k].view(abi.CLOCK_DTYPE)
+    return d
+
+
+def check(d, x, P, clk, world, n_eff, blob, tol, center_atol, map_rtol=1e-5, d_atol=1e-5):
+    assert int(n_eff) == int(d["n_eff"]) > 0
+    assert gp.rel_state(x, d["x"], d["x0"]) < tol, gp.rel_state(x, d["x"], d["x0"])
+    assert gp.rel_cov(P, d["P"]) < tol, gp.rel_cov(P, d["P"])
+    assert np.asarray(clk).tobytes() == d["clk"].tobytes()
+    err = np.abs(world[:, :3] - d["world"][:, :3])
+    assert (err <= gp.world_atol(d["world"])).all(), err.max()
+    np.testing.assert_array_equal(world[:, 3], d["world"][:, 3])
+    st = mapcmp.compare_digest(d["map1"], blob, rtol=map_rtol, center_atol=center_atol, d_atol=d_atol)
+    assert st["planes"] > 100
+
+
+def bucket_cfg(name):
+    return abi.CONFIGS["hilti" if name == "hilti" else "leg_fusion"]
+
+
+def test_fixtures_are_general():
+    """The fixtures carry what they are meant to exercise: a rotated, off-origin prior with negative keys, a dense P0 with
+    distinct attitude / position blocks and cross covariances, a skew part in the asymmetric one, a far-off scene."""
+    for name in BUCKETS:
+        d = load(f"ref_general_bucket_{name}.npz")
+        R = d["x0"]["rot"][0].reshape(3, 3)
+        assert np.abs(R - np.eye(3)).max() > 0.3
+        P = d["P0"].reshape(30, 30)
+        assert np.abs(P[:3, 3:6]).min() > 0 and np.abs(P[:6, 6:15]).min() > 0
+        assert len(set(np.round(np.diag(P)[:6], 12))) == 6
+        skew = np.abs(P - P.T).max() / np.abs(P).max()
+        assert (5e-7 < skew < 2e-6) if name == "asym" else skew == 0.0
+        assert (d["map1"]["key"] < 0).any()
+    far = load("ref_general_bucket_far.npz")
+    assert np.abs(far["x0"]["pos"][0][:2]).min() > 1500 and (far["map1"]["key"][:, 0] > 3000).all()
+
+
+@pytest.mark.parametrize("name", BUCKETS)
+@pytest.mark.parametrize("gain", [lko.GAIN_LITERAL, lko.GAIN_INFORMATION])
+def test_oracle_bucket_matches_general_golden(name, gain):
+    d = load(f"ref_general_bucket_{name}.npz")
+    cfg = bucket_cfg(name)
+    G = d["x0"]["rot"][0].reshape(3, 3)
+    o = lko.Oracle(cfg)
+    rot_cov, pos_cov = gp.map_covs(synth.exp_so3(gp.G_ROTVEC))
+    o.build_voxel_map(d["pw"], d["pb"], R=synth.exp_so3(gp.G_ROTVEC), rot_cov=rot_cov, pos_cov=pos_cov)
+    assert np.abs(G - synth.exp_so3(gp.G_ROTVEC)).max() < 0.02
+    mapcmp.compare_digest(d["map0"], o.map_export(), rtol=1e-7, center_atol=1e-12 * max(1.0, np.abs(d["pw"]).max()))
+    o.set_options(gain_mode=gain, iters=1, update_map=True)
+    o.set_filter(d["x0"], d["P0"], abi.process_cov_Q(cfg), d["clk0"])
+    r = o.predict_update_point(float(d["t"]), d["pts"])
+    x, P, _, clk = o.get_filter()
+    check(d, x, P, clk, r["world"], r["n_eff"], o.map_export(), 1e-10 if gain == lko.GAIN_LITERAL else 1e-7,
+          1e-9 * max(1.0, np.abs(d["pw"]).max() / 100))
+
+
+@pytest.mark.parametrize("kind", ["imu", "kin"])
+def test_oracle_stream_matches_general_golden(kind):
+    d = load(f"ref_general_stream_{kind}.npz")
+    cfg = abi.CONFIGS["leg_fusion"]
+    meas = d["meas"].view(abi.IMU_DTYPE if kind == "imu" else abi.KINIMU_DTYPE)
+    G = synth.exp_so3(gp.G_ROTVEC)
+    rot_cov, pos_cov = gp.map_covs(G)
+    o = lko.Oracle(cfg)
+    o.build_voxel_map(d["pw"], d["pb"], R=G, rot_cov=rot_cov, pos_cov=pos_cov)
+    mapcmp.compare_digest(d["map0"], o.map_export(), rtol=1e-7, center_atol=1e-12 * np.abs(d["pw"]).max())
+    o.set_options(gain_mode=lko.GAIN_LITERAL, iters=1, update_map=True, imu_mode_only=(kind == "imu"), gravity=9.81, acc_norm=9.79)
+    o.set_filter(d["x0"], d["P0"], abi.process_cov_Q(cfg), d["clk0"])
+    r = o.process_scan(float(d["begin"]), d["pts"], **{kind: meas})
+    x, P, _, clk = o.get_filter()
+    # the frame's map update refits planes from few points, where a state difference of STREAM_TOL moves d by ~1e-4
+    check(d, x, P, clk, r["world"], r["n_eff"], o.map_export(), gp.STREAM_TOL, 1e-6, map_rtol=1e-4, d_atol=1e-3)
+
+
+# ---- oracle against the compiled reference on random general priors ----------------------------------------------------
+
+from hypothesis import HealthCheck, given, settings  # noqa: E402
+from hypothesis import strategies as st  # noqa: E402
+
+
+@pytest.mark.skipif(not lkref.available(), reason="needs oracle/_ref/liblkref.so or /root/reference")
+@settings(max_examples=10, deadline=None, suppress_health_check=list(HealthCheck), derandomize=True)
+@given(seed=st.integers(0, 10**6), kin=st.booleans(), cfg_name=st.sampled_from(["leg_fusion", "hilti", "nclt", "diter"]),
+       asym=st.booleans(), far=st.booleans())
+def test_random_general_priors_match_reference(seed, kin, cfg_name, asym, far):
+    """One KILO::process frame after BuildVoxelMap from a general pose, reference vs oracle: attitude uniform on SO(3),
+    position within +-3 km (or +-60 m), a random dense SPD P0 (scaled, with a skew part when `asym`). The frame is one
+    bucket after the queue: across many buckets the map update at a dense prior amplifies rounding (see STREAM_TOL),
+    which would hide a layout or block mistake behind a loose tolerance."""
+    cfg = abi.CONFIGS[cfg_name]
+    g = np.random.default_rng(seed)
+    G = gp.so3_uniform(g)
+    pG = g.uniform(-3000.0, 3000.0, 3) if far else g.uniform(-60.0, 60.0, 3)
+    sc, pw, pb = gp.map_cloud(cfg, G, pG, stream=int(seed % 1000) + 1)
+    x0 = gp.prior_at(G, pG, g)
+    x0["vel"][0] = g.uniform(-0.5, 0.5, 3)
+    P0 = gp.dense_cov(g, scale=float(g.uniform(0.5, 1.5)))
+    if asym:
+        P0 = gp.skewed(P0, g)
+    clk = np.zeros(1, abi.CLOCK_DTYPE); clk["last_predict_time"] = 7.995; clk["last_update_time"] = 7.995
+    rot_cov, pos_cov = gp.map_covs(G)
+    o = lko.Oracle(cfg)
+    r = lkref.Reference(cfg, imu_mode_only=not kin, gravity=9.81, acc_norm=9.79)
+    o.set_options(gain_mode=lko.GAIN_LITERAL, iters=1, update_map=True, imu_mode_only=not kin, gravity=9.81, acc_norm=9.79)
+    for obj in (o, r):
+        obj.build_voxel_map(pw, pb, R=G, rot_cov=rot_cov, pos_cov=pos_cov)
+        obj.set_filter(x0, P0, abi.process_cov_Q(cfg), clk)
+    scan = gp.room_scan(cfg, sc, int(seed % 997) + 3, False, n_rings=8, n_az=100)
+    meas = (synth.kinimu_stream if kin else synth.imu_stream)(7.996, 8.13, stream=int(seed % 89) + 7)
+    out = r.process(8.0, 8.1, scan, **{"kin" if kin else "imu": meas})
+    assert out["ok"] and out["n_eff"] > 0.3 * len(scan)
+    ro = o.process_scan(8.0, out["body"], **{"kin" if kin else "imu": meas})
+    assert ro["n_eff"] == out["n_eff"]
+    err = np.abs(ro["world"][:, :3] - out["world"][:, :3])
+    assert (err <= gp.world_atol(out["world"], 3e-6)).all(), err.max()
+    assert (ro["world"][:, 3] == out["world"][:, 3]).all()
+    xo, Po, _, co = o.get_filter()
+    xr, Pr, _, cr = r.get_filter()
+    assert gp.rel_state(xo, xr, x0) < 1e-8, gp.rel_state(xo, xr, x0)
+    assert gp.rel_cov(Po, Pr) < 1e-8, gp.rel_cov(Po, Pr)
+    assert co.tobytes() == cr.tobytes()
+    # far from the origin, d = -n.c and the plane covariance carry the rounding of the normal times a lever arm of km
+    lever = max(1.0, np.abs(pG).max() / 30.0)
+    mapcmp.compare_blobs(r.map_export(), o.map_export(), rtol=1e-5 * lever, pt_atol=1e-10 * lever, var_rtol=1e-7 * lever,
+                         d_tol=1e-5 * lever)
