@@ -16,6 +16,13 @@ __device__ __forceinline__ void stall_note(uint32_t code, uint32_t detail) {
     }
 }
 
+// the global nanosecond timer, for the kernels' optional trace stamps
+__device__ __forceinline__ unsigned long long gtime() {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
+    return t;
+}
+
 // ---- mbarrier / bulk-copy primitives (PTX) ----------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {

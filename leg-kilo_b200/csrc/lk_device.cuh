@@ -97,6 +97,13 @@ struct ScanConst {
     double Ppp[6];  // sym(P[3:6,3:6]) upper
 };
 
+// The block's copy of one scan's constants, one double per thread; the caller synchronises before reading it.
+__device__ __forceinline__ void load_scan_const(ScanConst* dst, const ScanConst* src) {
+    const int tid = threadIdx.x;
+    if (tid < (int)(sizeof(ScanConst) / sizeof(double)))
+        reinterpret_cast<double*>(dst)[tid] = reinterpret_cast<const double*>(src)[tid];
+}
+
 // 32 doubles per chunk partial: A upper (21) | b (6) | sumR | count | pad
 constexpr int NACC = 29;
 constexpr int ACC_B = 21, ACC_SUMR = 27, ACC_CNT = 28;

@@ -32,11 +32,6 @@ namespace lk {
 
 namespace {
 
-__device__ __forceinline__ unsigned long long gtime() {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-    return t;
-}
 #define FT(slot) do { if (a.trace && threadIdx.x == 0 && (slot) < 32) a.trace[(size_t)blockIdx.x * 32 + (slot)] = gtime(); } while (0)
 // per-iteration stamps of the first three exchanges i: 14 + i pass done, 2 + 4i block row in shared memory, 3 + 4i all-reduce
 // total in shared memory, 4 + 4i solve done (tools/trace_fused.py)
@@ -351,15 +346,14 @@ template <bool OBS, bool INL, bool INS>
 cudaError_t launch_one(const FusedArgs& a, const FusedInline* inl, uint32_t grid, cudaStream_t s, int mode) {
     auto kern = k_scan_fused<OBS, INL, INS>;
     constexpr size_t SMEM = INS ? sizeof(FusedSmemIns) : sizeof(FusedSmem);
-    static bool attr[64];
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev >= 0 && dev < 64 && !attr[dev]) {
+    static PerDeviceOnce once;
+    if (once.first()) {
+        int dev = 0;
+        cudaGetDevice(&dev);
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM);
         if (e != cudaSuccess) return e;
         e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, carveout_percent(SMEM, dev));
         if (e != cudaSuccess) return e;
-        attr[dev] = true;
     }
     typename InlineSel<INL>::type local_inl;
     const typename InlineSel<INL>::type* ip;

@@ -16,6 +16,7 @@
 #include "lk_kernels.h"
 #include "lk_mapdev.h"
 #include "lk_insert.cuh"
+#include "lk_point.cuh"
 
 namespace lk {
 
@@ -46,19 +47,15 @@ __global__ void __launch_bounds__(256) k_insert_p1(const __grid_constant__ Inser
     __shared__ ScanConst s_sc;
     const int tid = threadIdx.x;
     const ChunkDesc cd = a.chunks[a.chunk_first + blockIdx.x];
-    if (tid < (int)(sizeof(ScanConst) / sizeof(double)))
-        reinterpret_cast<double*>(&s_sc)[tid] = reinterpret_cast<const double*>(a.sc + cd.scan)[tid];
+    load_scan_const(&s_sc, a.sc + cd.scan);
     __syncthreads();
     const Globals& g = a.g;
     MapDev md = a.md;
     for (uint32_t i = tid; i < cd.count; i += blockDim.x) {
-        const float4 pt = __ldg(a.pts + cd.start + i);
-        const double bx = pt.x, by = pt.y, bz0 = pt.z;
-        const double pix = g.Re[0] * bx + g.Re[1] * by + g.Re[2] * bz0 + g.te[0];
-        const double piy = g.Re[3] * bx + g.Re[4] * by + g.Re[5] * bz0 + g.te[1];
-        const double piz = g.Re[6] * bx + g.Re[7] * by + g.Re[8] * bz0 + g.te[2];
+        PointCtx pc;
+        body_point(__ldg(a.pts + cd.start + i), g, pc);
         DevPoint p;
-        make_insert_point(pix, piy, piz, bx, by, (bz0 == 0.0) ? 0.0001 : bz0, s_sc, g, p);  // calcBodyCov saw pb.z == 0 -> 1e-4
+        make_insert_point(pc.pix, pc.piy, pc.piz, pc.pbx, pc.pby, pc.pbz, s_sc, g, p);
         const uint32_t li = cd.start + i - a.pt_base;
         a.ipts[li] = p;
         if (a.world) {

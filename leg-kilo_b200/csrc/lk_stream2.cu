@@ -95,8 +95,7 @@ __global__ void __launch_bounds__(S2_THREADS, 2) k_residual_stream2(const __grid
     S2Smem<S2_WARPS>* sm = reinterpret_cast<S2Smem<S2_WARPS>*>(s_raw);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const ChunkDesc cd = a.chunks[a.chunk_first + blockIdx.x];
-    if (tid < (int)(sizeof(ScanConst) / sizeof(double)))
-        reinterpret_cast<double*>(&sm->sc)[tid] = reinterpret_cast<const double*>(a.sc + cd.scan)[tid];
+    load_scan_const(&sm->sc, a.sc + cd.scan);
     __syncthreads();
     const ScanConst& sc = sm->sc;
     const MapView mv = {a.slots, a.hash_mask, a.nodes, a.hot};
@@ -210,15 +209,7 @@ __global__ void __launch_bounds__(S2_THREADS, 2) k_residual_stream2(const __grid
     for (int i = 0; i < 6; ++i) acc[ACC_B + i] = rest[i];
     acc[ACC_SUMR] = rest[6];
     acc[ACC_CNT] = rest[7];
-    const double tot = warp_transpose_sum(acc, lane);
-    sm->slice[warp * 32 + lane] = tot;
-    __syncthreads();
-    if (tid < 32) {
-        double v = 0.0;
-#pragma unroll
-        for (int w2 = 0; w2 < S2_WARPS; ++w2) v += sm->slice[w2 * 32 + tid];
-        a.partial[(size_t)(a.chunk_first + blockIdx.x) * PARTIAL_STRIDE + tid] = v;
-    }
+    block_row<S2_WARPS>(acc, sm->slice, [&](int i, double v) { a.partial[(size_t)(a.chunk_first + blockIdx.x) * PARTIAL_STRIDE + i] = v; });
 }
 
 // The points the pipelined kernel could not finish on the hot images — no plane in the home node (octree descent, voxel_map.cc:412-424)
@@ -245,15 +236,14 @@ constexpr int FB_THREADS = 128;
 __global__ void __launch_bounds__(FB_THREADS, 8) k_residual_fallback(const __grid_constant__ ResidualArgs a) {
     __shared__ ScanConst s_sc;
     __shared__ double s_slice[(FB_THREADS / 32) * 32];
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int tid = threadIdx.x;
     const uint32_t c = a.chunk_first + blockIdx.x;
     uint32_t cnt[S2_FB_WARPS], total = 0;
 #pragma unroll
     for (uint32_t w = 0; w < S2_FB_WARPS; ++w) { cnt[w] = __ldg(a.fb_cnt + (size_t)c * S2_FB_WARPS + w); total += cnt[w]; }
     if (total == 0) return;  // the same for every thread of the block
     const ChunkDesc cd = a.chunks[c];
-    if (tid < (int)(sizeof(ScanConst) / sizeof(double)))
-        reinterpret_cast<double*>(&s_sc)[tid] = reinterpret_cast<const double*>(a.sc + cd.scan)[tid];
+    load_scan_const(&s_sc, a.sc + cd.scan);
     __syncthreads();
     const MapView mv = {a.slots, a.hash_mask, a.nodes, a.hot};
     const float4* __restrict__ pts = a.pts + cd.start;
@@ -270,18 +260,10 @@ __global__ void __launch_bounds__(FB_THREADS, 8) k_residual_fallback(const __gri
         Row row;
         // bit 15: the home voxel is a plane that gated the point out — build_single_residual left is_success false there
         // (voxel_map.cc:370-411), so only the neighbour voxel is left to try; otherwise the whole sequence, descent included
-        const bool ok = (ent & 0x8000u) ? point_row_neighbour(pt, s_sc, mv, a.g, row) : point_row(pt, s_sc, mv, a.g, row, nullptr);
+        const bool ok = (ent & 0x8000u) ? point_row_neighbour(pt, s_sc, mv, a.g, row) : point_row(pt, s_sc, mv, a.g, row);
         if (ok) accumulate_row(row, acc);
     }
-    const double tot = warp_transpose_sum(acc, lane);
-    s_slice[warp * 32 + lane] = tot;
-    __syncthreads();
-    if (tid < 32) {
-        double v = 0.0;
-#pragma unroll
-        for (int w2 = 0; w2 < FB_THREADS / 32; ++w2) v += s_slice[w2 * 32 + tid];
-        a.partial[(size_t)c * PARTIAL_STRIDE + tid] += v;
-    }
+    block_row<FB_THREADS / 32>(acc, s_slice, [&](int i, double v) { a.partial[(size_t)c * PARTIAL_STRIDE + i] += v; });
 }
 
 }  // namespace

@@ -3,6 +3,7 @@ instructions that prove the memory path (UBLKCP = 1-D TMA bulk copy, LDGSTS = cp
 
     python tools/sass_stats.py [LIB] [--json]
     python tools/sass_stats.py [LIB] --local SUBSTRING
+    python tools/sass_stats.py --diff OLD_LIB NEW_LIB
 
 --local lists the local-memory instructions (STL / LDL: stack frame and register spills) of every kernel whose mangled or
 demangled name contains SUBSTRING, counted per source file and line. The library is built with -lineinfo, so nvdisasm
@@ -50,8 +51,41 @@ def local_report(so, pat):
     return res
 
 
+def sass_by_function(so):
+    """{mangled name, anonymous-namespace hash normalised: ([opcode of every instruction], [every SASS line])}"""
+    txt = subprocess.run(["cuobjdump", "-sass", so], capture_output=True, text=True, check=True).stdout
+    anon = lambda m: "%d_GLOBAL__N__%s" % (len("_GLOBAL__N__" + m.group(1)), m.group(1))  # keeps the name demangleable
+    txt = re.sub(r'\d+_GLOBAL__N__[0-9a-f]{8}_\d+_(\w+?_cu)_[0-9a-f]{8}', anon, txt)
+    res, name = collections.OrderedDict(), None
+    for l in txt.splitlines():
+        m = re.search(r'Function : (\S+)', l)
+        if m:
+            name = m.group(1); res[name] = ([], []); continue
+        if name is None: continue
+        res[name][1].append(l.strip())
+        m = re.match(r'\s+/\*[0-9a-f]{4,}\*/\s+(?:@!?U?P\d+\s+)?([A-Z0-9_.]+)', l)
+        if m: res[name][0].append(m.group(1))
+    return res
+
+
+def diff(old_so, new_so):
+    old, new = sass_by_function(old_so), sass_by_function(new_so)
+    same = 0
+    for k in list(old) + [k for k in new if k not in old]:
+        if k in old and k in new and old[k][1] == new[k][1]:
+            same += 1; continue
+        n_old, n_new = (len(d[k][0]) if k in d else None for d in (old, new))
+        ops = "only in " + ("new" if n_old is None else "old") if None in (n_old, n_new) else \
+            "same opcodes" if collections.Counter(old[k][0]) == collections.Counter(new[k][0]) else "opcodes differ"
+        print("%-70s %6s -> %-6s %s" % (short(k)[:70], n_old, n_new, ops))
+    print("%d of %d functions byte-identical" % (same, len(set(old) | set(new))))
+
+
 def main():
     args = sys.argv[1:]
+    if "--diff" in args:
+        i = args.index("--diff")
+        return diff(args[i + 1], args[i + 2])
     pat = None
     if "--local" in args:
         i = args.index("--local")
@@ -75,16 +109,9 @@ def main():
                 for (f, ln) in sorted(lines):
                     print("    %-24s %5d   STL %3d  LDL %3d" % (f, ln, lines[(f, ln)]["STL"], lines[(f, ln)]["LDL"]))
         return
-    txt = subprocess.run(["cuobjdump", "-sass", so], capture_output=True, text=True).stdout
-    name = None; cnt = collections.OrderedDict(); ops = {}
-    for l in txt.splitlines():
-        m = re.search(r'Function : (\S+)', l)
-        if m:
-            name = m.group(1); cnt[name] = 0; ops[name] = collections.Counter(); continue
-        m = re.match(r'\s+/\*[0-9a-f]{4,}\*/\s+(?:@!?U?P\d+\s+)?([A-Z0-9_.]+)', l)
-        if name and m:
-            cnt[name] += 1
-            ops[name][m.group(1).split('.')[0]] += 1
+    sass = sass_by_function(so)
+    cnt = collections.OrderedDict((k, len(v[0])) for k, v in sass.items())
+    ops = {k: collections.Counter(op.split('.')[0] for op in v[0]) for k, v in sass.items()}
     rows = []
     KEYS = ["UBLKCP", "UTMALDG", "LDGSTS", "SYNCS", "DFMA", "DMUL", "DADD", "SHFL", "LDG", "STG", "LDS", "STS", "BAR", "ATOMG", "RED", "MUFU", "CALL"]
     for k, v in sorted(cnt.items(), key=lambda kv: -kv[1]):
