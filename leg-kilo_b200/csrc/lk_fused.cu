@@ -38,6 +38,15 @@ namespace {
 #define FTI(slot) do { if (it_global < 3) FT(slot); } while (0)
 // per-bucket stamps of the streaming variants (block 0, first 64 buckets, 8 stamps each, behind the per-block area)
 #define FTS(slot) do { if (a.trace && blockIdx.x == 0 && threadIdx.x == 0 && k < 64) a.trace[(size_t)gridDim.x * 32 + (size_t)k * 8 + (slot)] = gtime(); } while (0)
+// The all-reduce's hop stamps and poll-round counts (lk_llsync.cuh: LL_HOP_SLOTS per exchange, first three exchanges, 16
+// slots per block behind the per-bucket area: 160 blocks fill the 8192-stamp trace area). Unlike FT / FTI they are gated at
+// compile time as well as by a.trace: only `make HOP_TRACE=1` (a library of its own, tools/trace_fused.py --hops) compiles
+// them in, so the default library's all-reduce has the same instructions whether tracing exists or not.
+#ifndef LK_HOP_TRACE
+#define LK_HOP_TRACE 0
+#endif
+#define FT_HOPS() ((LK_HOP_TRACE && a.trace && it_global < 3) \
+                       ? a.trace + (size_t)gridDim.x * 32 + 64 * 8 + (size_t)blockIdx.x * 16 + it_global * LL_HOP_SLOTS : nullptr)
 
 constexpr int BLOCK = FB;
 constexpr int WARPS = BLOCK / 32;
@@ -257,7 +266,7 @@ __global__ void __launch_bounds__(BLOCK, 1) k_scan_fused(const __grid_constant__
 #pragma unroll
                 for (int w = 0; w < WARPS; ++w) v += sm->slice[w * 32 + lane];
                 if (!dep_waited) asm volatile("griddepcontrol.wait;" ::: "memory");  // the rows / outputs of the previous launch
-                sm->f.acc[lane] = ll_allreduce(a.ll, it_global & 1u, a.epoch + it_global, blockIdx.x, n_chunks, v, lane);
+                sm->f.acc[lane] = ll_allreduce(a.ll, it_global & 1u, a.epoch + it_global, blockIdx.x, n_chunks, v, lane, FT_HOPS());
             }
             dep_waited = true;
             __syncthreads();

@@ -8,6 +8,16 @@
 // iteration parity (a block writes iteration i+2 only after it has seen every row of iteration i+1,
 // i.e. after every block has finished reading iteration i).
 //
+// Every group row is published in LL_REPLICAS copies, and block b polls only copy b % LL_REPLICAS, so
+// each copy's lines have ~blocks / LL_REPLICAS readers instead of all of them. The reuse rule above holds
+// for every copy, for every block that publishes a chunk row in exchange i+1: a leader writes all copies of
+// its group row of i+2 at one point of its program, after it has seen (in its own copy) every group row of
+// i+1; each of those exists only once its group's leader has seen every chunk row of that group for i+1, and
+// a block publishes its chunk row of i+1 only after it has read its copy of every group row of i. Which copy
+// a block reads plays no part in that chain. A block with b >= n_chunks of exchange i+1 publishes nothing
+// there, so the chain does not order its reads of i before the writes of i+2; it only holds because such a
+// block would have to lag a whole pass and solve behind the others. This is as old as the two buffers.
+//
 // Summation order (shared with the multi-kernel path, lk_solve.cuh: block_sum_partials):
 //   total = sum over groups g ascending of ( sum over the rows of group g ascending ),
 //   group g = chunks [g*LK_GROUP, (g+1)*LK_GROUP) of the bucket — a function of the bucket alone.
@@ -15,24 +25,30 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "lk_async.cuh"
+
 namespace lk {
 
 constexpr int LK_GROUP = 8;          // chunk rows per group (level-1 fan-in)
 constexpr int LL_ROW = 32;           // slots (doubles) per row
 constexpr int LL_MAX_CHUNKS = 160;   // >= SM count: the fused kernel runs one chunk per block
 constexpr int LL_MAX_GROUPS = (LL_MAX_CHUNKS + LK_GROUP - 1) / LK_GROUP;
+constexpr int LL_REPLICAS = 4;       // copies of every group row (level-2 readers per copy: blocks / LL_REPLICAS)
 
 struct LLView {
     ulonglong2* chunk_rows;  // [2][LL_MAX_CHUNKS][LL_ROW]
-    ulonglong2* group_rows;  // [2][LL_MAX_GROUPS][LL_ROW]
+    ulonglong2* group_rows;  // [2][LL_REPLICAS][LL_MAX_GROUPS][LL_ROW]
     uint32_t* stall;         // [8] watchdog record: [0] != 0 once a poll gave up | block | tag | first row | rows | lane
 };
-constexpr size_t LL_ROWS_BYTES = (size_t)2 * (LL_MAX_CHUNKS + LL_MAX_GROUPS) * LL_ROW * sizeof(ulonglong2);
+constexpr size_t LL_ROWS_BYTES = (size_t)2 * (LL_MAX_CHUNKS + LL_REPLICAS * LL_MAX_GROUPS) * LL_ROW * sizeof(ulonglong2);
 constexpr size_t LL_BYTES = LL_ROWS_BYTES + 64;
 // A poll that sees nothing for this many rounds (seconds) gives up, records who waited for what and lets the kernel run
 // to its end with garbage sums; the host then reports LK_ERR_CUDA instead of hanging. It means the blocks of the grid were
 // not all resident (another process holds SMs: see INTEGRATION.md "Sharing a device") — or a bug.
 constexpr uint32_t LL_SPIN_LIMIT = 1u << 23;
+// Slots per exchange of the optional hop trace (ll_allreduce's `hops`): [0] own chunk row stored (a leader: level 1 entered),
+// [1] level-1 sum complete (leader), [2] group row stored (leader), [3] total in hand, [4] poll rounds: level 1 | level 2 << 32
+constexpr int LL_HOP_SLOTS = 5;
 
 __device__ __forceinline__ void ll_store(ulonglong2* p, double v, uint32_t tag) {
     const unsigned long long b = (unsigned long long)__double_as_longlong(v);
@@ -41,38 +57,71 @@ __device__ __forceinline__ void ll_store(ulonglong2* p, double v, uint32_t tag) 
     asm volatile("st.relaxed.gpu.global.v2.u64 [%0], {%1, %2};" ::"l"(p), "l"(w0), "l"(w1) : "memory");
 }
 
+// Gives up a poll: records who waited for what (the first to give up) so the host can report it.
+__device__ __forceinline__ void ll_give_up(uint32_t* stall, uint32_t tag, uint32_t r0, uint32_t n, int lane) {
+    if (atomicCAS(stall, 0u, 1u) == 0u) {
+        stall[1] = blockIdx.x; stall[2] = tag; stall[3] = r0; stall[4] = n; stall[5] = (uint32_t)lane;
+        __threadfence();
+    }
+}
+
 // Element `lane` of rows [r0, r0 + n) (n <= N), summed in ascending row order starting from 0.0. Every poll round
-// issues ALL n loads back to back (independent, so they overlap in the memory system: one L2 round trip per round,
-// not one per row) and only then inspects the tags; the round repeats until every row carries the tag (rows never
-// change once published within an epoch, so re-reading the ones that already matched is harmless). One full warp.
-template <int N>
+// issues its loads back to back (independent, so they overlap in the memory system: one L2 round trip per round, not one
+// per row) and only then inspects the tags. KEEP = false: every round reloads every row. KEEP = true: a row that matched
+// keeps its words and is not loaded again (rows never change once published within an epoch), so a round loads only the
+// rows still missing. The level-1 poll of a group leader (<= 7 rows, one reader per row) reloads: keeping its words
+// across rounds costs the per-scan kernel spill stores and stack frame, and its rows have no other readers to slow down.
+// `rounds` receives the number of poll rounds. One full warp.
+template <int N, bool KEEP>
 __device__ __forceinline__ double ll_sum_rows(const ulonglong2* rows, uint32_t r0, uint32_t n, uint32_t tag, int lane,
-                                              uint32_t* stall, double first = 0.0, bool have_first = false) {
+                                              uint32_t* stall, uint32_t& rounds, double first = 0.0, bool have_first = false) {
+    static_assert(N <= 32, "one bit per row");
     const ulonglong2* p = rows + (size_t)r0 * LL_ROW + lane;
     unsigned long long w0[N], w1[N];
     const unsigned long long want = ((unsigned long long)tag << 32);
-    bool all;
     uint32_t spins = 0;
-    do {
+    if constexpr (!KEEP) {
+        bool all;
+        do {
 #pragma unroll
-        for (int k = 0; k < N; ++k)
-            if ((uint32_t)k < n && !(have_first && k == 0))
-                asm volatile("ld.relaxed.gpu.global.v2.u64 {%0, %1}, [%2];" : "=l"(w0[k]), "=l"(w1[k]) : "l"(p + (size_t)k * LL_ROW));
-        all = true;
+            for (int k = 0; k < N; ++k)
+                if ((uint32_t)k < n && !(have_first && k == 0))
+                    asm volatile("ld.relaxed.gpu.global.v2.u64 {%0, %1}, [%2];" : "=l"(w0[k]), "=l"(w1[k]) : "l"(p + (size_t)k * LL_ROW));
+            all = true;
 #pragma unroll
-        for (int k = 0; k < N; ++k)
-            if ((uint32_t)k < n && !(have_first && k == 0))
-                all = all && ((w0[k] & 0xffffffff00000000ull) == want) && ((w1[k] & 0xffffffff00000000ull) == want);
-        if (!all && ((++spins & 0xfffu) == 0u)) {  // watchdog, off the fast path
-            if (spins >= LL_SPIN_LIMIT || *reinterpret_cast<volatile uint32_t*>(stall) != 0u) {
-                if (atomicCAS(stall, 0u, 1u) == 0u) {
-                    stall[1] = blockIdx.x; stall[2] = tag; stall[3] = r0; stall[4] = n; stall[5] = (uint32_t)lane;
-                    __threadfence();
+            for (int k = 0; k < N; ++k)
+                if ((uint32_t)k < n && !(have_first && k == 0))
+                    all = all && ((w0[k] & 0xffffffff00000000ull) == want) && ((w1[k] & 0xffffffff00000000ull) == want);
+            ++spins;
+            if (!all && ((spins & 0xfffu) == 0u)) {  // watchdog, off the fast path
+                if (spins >= LL_SPIN_LIMIT || *reinterpret_cast<volatile uint32_t*>(stall) != 0u) {
+                    ll_give_up(stall, tag, r0, n, lane);
+                    break;
                 }
-                break;
+            }
+        } while (!all);
+    } else {
+        uint32_t todo = (n >= 32u ? 0xffffffffu : (1u << n) - 1u) & (have_first ? ~1u : ~0u);  // rows not seen yet
+        while (true) {
+#pragma unroll
+            for (int k = 0; k < N; ++k)
+                if ((todo >> k) & 1u)
+                    asm volatile("ld.relaxed.gpu.global.v2.u64 {%0, %1}, [%2];" : "=l"(w0[k]), "=l"(w1[k]) : "l"(p + (size_t)k * LL_ROW));
+#pragma unroll
+            for (int k = 0; k < N; ++k)
+                if (((todo >> k) & 1u) && ((w0[k] & 0xffffffff00000000ull) == want) && ((w1[k] & 0xffffffff00000000ull) == want))
+                    todo &= ~(1u << k);
+            ++spins;
+            if (todo == 0u) break;
+            if ((spins & 0xfffu) == 0u) {  // watchdog, off the fast path
+                if (spins >= LL_SPIN_LIMIT || *reinterpret_cast<volatile uint32_t*>(stall) != 0u) {
+                    ll_give_up(stall, tag, r0, n, lane);
+                    break;
+                }
             }
         }
-    } while (!all);
+    }
+    rounds = spins;
     double s = 0.0;
 #pragma unroll
     for (int k = 0; k < N; ++k)
@@ -86,23 +135,40 @@ __device__ __forceinline__ double ll_sum_rows(const ulonglong2* rows, uint32_t r
 // The all-reduce. `v` = this block's row element `lane` (warp 0 calls, all 32 lanes). Block b owns
 // chunk b of the n_chunks chunks of the bucket (blocks with b >= n_chunks contribute nothing but still receive the
 // total). Returns the total of element `lane` in the fixed grouped order. Level 1: rows travel through global memory in
-// the flagged format, the group's first block adds them; level 2: it publishes the group row, every block polls the
-// (<= 20) group rows.
+// the flagged format, the group's first block adds them; level 2: it publishes the group row in LL_REPLICAS copies, every
+// block polls its copy of the (<= 20) group rows. `hops` (nullptr: no trace) receives LL_HOP_SLOTS stamps and counts.
 __device__ __forceinline__ double ll_allreduce(const LLView& ll, uint32_t parity, uint32_t tag, uint32_t b, uint32_t n_chunks,
-                                               double v, int lane) {
+                                               double v, int lane, unsigned long long* hops = nullptr) {
+    constexpr size_t COPY = (size_t)LL_MAX_GROUPS * LL_ROW;
     ulonglong2* crows = ll.chunk_rows + (size_t)parity * LL_MAX_CHUNKS * LL_ROW;
-    ulonglong2* grows = ll.group_rows + (size_t)parity * LL_MAX_GROUPS * LL_ROW;
+    ulonglong2* grows = ll.group_rows + (size_t)parity * LL_REPLICAS * COPY;
     const uint32_t n_groups = (n_chunks + LK_GROUP - 1) / LK_GROUP;
+    uint32_t r1 = 0, r2 = 0;
     if (b < n_chunks) {
         if ((b % LK_GROUP) == 0) {
+            if (hops && lane == 0) hops[0] = gtime();
             const uint32_t n = min((uint32_t)LK_GROUP, n_chunks - b);
-            const double s = ll_sum_rows<LK_GROUP>(crows, b, n, tag, lane, ll.stall, v, true);
-            ll_store(grows + (size_t)(b / LK_GROUP) * LL_ROW + lane, s, tag);
+            const double s = ll_sum_rows<LK_GROUP, false>(crows, b, n, tag, lane, ll.stall, r1, v, true);
+            if (hops && lane == 0) hops[1] = gtime();
+            ulonglong2* g = grows + (size_t)(b / LK_GROUP) * LL_ROW + lane;
+#pragma unroll
+            for (int r = 0; r < LL_REPLICAS; ++r) ll_store(g + (size_t)r * COPY, s, tag);
+            if (hops && lane == 0) hops[2] = gtime();
         } else {
             ll_store(crows + (size_t)b * LL_ROW + lane, v, tag);
+            if (hops && lane == 0) hops[0] = gtime();
         }
     }
-    return ll_sum_rows<LL_MAX_GROUPS>(grows, 0, n_groups, tag, lane, ll.stall);
+    const double t = ll_sum_rows<LL_MAX_GROUPS, true>(grows + (size_t)(b % LL_REPLICAS) * COPY, 0, n_groups, tag, lane, ll.stall, r2);
+    if (hops) {
+        r1 = __reduce_max_sync(0xffffffffu, r1);
+        r2 = __reduce_max_sync(0xffffffffu, r2);
+        if (lane == 0) {
+            hops[3] = gtime();
+            hops[4] = (unsigned long long)r1 | ((unsigned long long)r2 << 32);
+        }
+    }
+    return t;
 }
 
 }  // namespace lk

@@ -1,6 +1,6 @@
 """Per-phase %globaltimer trace of the fused per-scan kernel at the headline shape (latency diagnosis).
 
-  python tools/trace_fused.py [--workload leg_fusion_b1] [--scans 512] [--launches 48] [name=value ...]
+  python tools/trace_fused.py [--workload leg_fusion_b1] [--scans 512] [--launches 48] [--hops] [name=value ...]
 
 Builds bench.py's workload (by default leg_fusion_b1 with its 512-scan ring: inputs larger than L2), warms the ring up
 once, then issues --launches back-to-back launches exactly as bench.py does (kernel_timing = 0, so consecutive launches
@@ -11,6 +11,12 @@ Stamps per block (slots, see lk_fused.cu): 0 entry, 1 first pass starts, per ite
 31 end; a build without the pass-done and re-projection stamps gets the combined phases printed instead. Times in
 microseconds: medians over the traced launches (min and max beside them) of per-launch medians over blocks, unless the
 name says "slowest block" or "last block".
+
+--hops runs the library built with `make -C leg-kilo_b200/csrc HOP_TRACE=1`, whose all-reduce also stamps, per block and
+exchange, its chunk row stored (a group leader: level 1 entered), the leader's level-1 sum complete and group row stored, the
+total in hand, and its poll rounds per level (lk_llsync.cuh: LL_HOP_SLOTS). Hop 1 runs from the slowest chunk row of a group
+to that group's row stored; hop 2 from the last group row stored to the total in hand, for the median and the slowest block.
+Poll rounds are the most any lane of the warp took.
 """
 import argparse
 import os
@@ -23,9 +29,11 @@ for p in ("leg-kilo_b200/python", "tests"):
     sys.path.insert(0, os.path.join(ROOT, p))
 sys.path.insert(0, ROOT)
 import bench  # noqa: E402
+import legkilo_b200  # noqa: E402
 from legkilo_b200 import Engine, _p, abi, lib  # noqa: E402
 
 TRACE_AREA, TRACE_AREAS = 8192, 64  # lk_api.cu
+HOP_SLOTS, GROUP = 5, 8  # lk_llsync.cuh: LL_HOP_SLOTS, LK_GROUP
 
 
 def main():
@@ -33,8 +41,12 @@ def main():
     ap.add_argument("--workload", default="leg_fusion_b1")
     ap.add_argument("--scans", type=int, default=0, help="ring size (default: bench.py's)")
     ap.add_argument("--launches", type=int, default=48)
+    ap.add_argument("--hops", action="store_true", help="load the hop-trace library (make -C leg-kilo_b200/csrc HOP_TRACE=1) "
+                    "and split the all-reduce into its two hops")
     ap.add_argument("param", nargs="*", help="engine parameter name=value (lk_set_param)")
     args = ap.parse_args()
+    if args.hops:
+        legkilo_b200.LIB_PATH = os.path.join(os.path.dirname(legkilo_b200.LIB_PATH), "liblegkilo_b200_hops.so")
     L = min(args.launches, TRACE_AREAS)
     w = bench.WORKLOADS[args.workload]
     assert w["batch"] == 1, "the fused kernel runs batch-of-one workloads"
@@ -62,9 +74,15 @@ def main():
     eng.set_param("trace", 0)
     offs = wl["offs"]
     T = []
+    H = [] if args.hops else None
     for j, s in enumerate(scans):
         nb = int((offs[s + 1] - offs[s] + 255) // 256)
         T.append(tr[j * TRACE_AREA: j * TRACE_AREA + nb * 32].reshape(nb, 32).astype(np.int64))
+        if args.hops:
+            h0 = j * TRACE_AREA + nb * 32 + 64 * 8
+            H.append(tr[h0: h0 + nb * 16].reshape(nb, 16).astype(np.int64))
+    if args.hops and not any(h.any() for h in H):
+        sys.exit("%s wrote no hop stamps: it was built without LK_HOP_TRACE" % legkilo_b200.LIB_PATH)
     it_n = w["iters"]
     us = 1e-3
 
@@ -95,6 +113,19 @@ def main():
             put("it%d all-reduce: done after last block row" % it, (np.median(b[:, s_ar]) - last_in) * us)
             put("it%d solve (-> next pass)" % it, np.median(b[:, s_sol] - b[:, s_ar]) * us)
             prev = b[:, s_sol]
+            if H is not None:
+                h = H[j][:, it * HOP_SLOTS: (it + 1) * HOP_SLOTS]
+                lead = np.arange(0, h.shape[0], GROUP)
+                last_row = np.array([h[g: g + GROUP, 0].max() for g in lead])  # slowest chunk row of each group (leader: entry)
+                put("it%d hop 1: slowest chunk row -> group row stored (median group)" % it, np.median(h[lead, 2] - last_row) * us)
+                put("it%d hop 1: slowest chunk row -> group row stored (slowest group)" % it, (h[lead, 2] - last_row).max() * us)
+                put("it%d hop 1: of which level-1 sum -> group row stored" % it, np.median(h[lead, 2] - h[lead, 1]) * us)
+                put("it%d hop 2: last group row stored -> total in hand (median block)" % it, (np.median(h[:, 3]) - h[lead, 2].max()) * us)
+                put("it%d hop 2: last group row stored -> total in hand (slowest block)" % it, (h[:, 3].max() - h[lead, 2].max()) * us)
+                put("it%d poll rounds hop 1 (median leader)" % it, np.median(h[lead, 4] & 0xffffffff))
+                put("it%d poll rounds hop 1 (most)" % it, (h[lead, 4] & 0xffffffff).max())
+                put("it%d poll rounds hop 2 (median block)" % it, np.median(h[:, 4] >> 32))
+                put("it%d poll rounds hop 2 (most)" % it, (h[:, 4] >> 32).max())
         if has(b, 20):
             put("re-projection", np.median(b[:, 20] - prev) * us)
             put("after re-projection -> loop left", np.median(b[:, 30] - b[:, 20]) * us)
