@@ -228,6 +228,21 @@ int lk_map_download(lk_handle h, void* blob, size_t capacity, size_t* bytes_out)
  * xyz_world = feats_down_world_ (float xyz, n*3), xyz_body = feats_down_body_ (lidar frame). */
 int lk_map_build(lk_handle h, const float* xyz_world, const float* xyz_body, size_t n,
                  const double rot[9], const double rot_cov[9], const double pos_cov[9]);
+/* Step 4 of KILO::predictUpdatePoint (KILO.cc:216-231) without the filter: UpdateVoxelMap (voxel_map.cc:336-361) of
+ * n_sets point sets, each placed at its own pose. Set s holds pts[set_offsets[s] .. set_offsets[s+1]) (float4, lidar frame,
+ * the 4th component ignored) and is placed with rot[9s..] (row-major body->world), pos[3s..], rot_cov[9s..] and
+ * pos_cov[9s..] (the theta and position blocks of P, row-major 3x3):
+ *   p_i = R_ext p_b + t_ext, p_w = R p_i + p, var = (R R_ext) Sigma_b (R R_ext)^T + (R [p_i]x) rot_cov (R [p_i]x)^T + pos_cov.
+ * rot_cov / pos_cov enter through their symmetric parts 0.5 (a_ij + a_ji), as the filter's P blocks do in streaming: a set
+ * given the state and P a streaming bucket ended with is placed bitwise as that bucket's insert placed it.
+ * Points are inserted in set order, then in their order within the set, exactly as consecutive UpdateVoxelMap calls would.
+ * A handle with no map starts from an empty one (as streaming from empty does). This is not lk_map_build: BuildVoxelMap
+ * fits each root once after all points, and UpdateVoxelMap refits as points arrive.
+ * LK_ERR_INVALID_ARG: a NULL argument with n_sets > 0, set_offsets not monotone, or a non-finite entry of rot, pos, rot_cov
+ * or pos_cov. n_sets == 0 does nothing. LK_ERR_CAPACITY: the map pools ran out (the map then holds the points inserted up
+ * to the window that overflowed, and some of that window's). A staged batch stays staged. */
+int lk_map_insert(lk_handle h, uint32_t n_sets, const float* pts, const uint32_t* set_offsets, const double* rot,
+                  const double* pos, const double* rot_cov, const double* pos_cov);
 /* Map counters: out[0]=roots, out[1]=nodes, out[2]=retained points, out[3]=plane nodes. */
 int lk_map_stats(lk_handle h, uint64_t out[4]);
 /* VoxelMapManager::mapSliding + clearMemOutOfMap (voxel_map.cc:552-594; dead code in the reference, needed for unbounded

@@ -97,6 +97,9 @@ struct lk_context {
     DevBuf dbg_ok, dbg_h, dbg_z, dbg_R, dbg_key, tmp, trace, bar;
     DevBuf ins_pts, ins_root, ins_pend, ins_touched, ins_counters, ins_list;
     uint64_t ins_pend_nodes = 0;
+    // lk_map_insert: one window's points, chunk table + placements (mi_small, staged in h_mi), and insert scratch
+    DevBuf mi_pts, mi_small, mi_ipts, mi_root, mi_touched, mi_counters, mi_list;
+    PinnedBuf h_mi;
     int trace_on = 0;
     uint32_t trace_seq = 0;  // fused launches traced since the trace was switched on or last read back
     int lane_cache = 1;
@@ -995,6 +998,49 @@ static int run_kernels(lk_handle h, uint32_t first, uint32_t count, int iters, b
     return LK_OK;
 }
 
+// Before an UpdateVoxelMap of up to n points (which may create the map): room for them in the pools, what earlier
+// launches freed made available (push_counters), and the per-root pending counts of the insert sized to the node pool.
+static int insert_headroom(lk_handle h, uint64_t n) {
+    cudaStream_t s = h->stream;
+    int rc = h->map.ready() ? h->map.sync_counters(s, h->err) : LK_OK;
+    // Worst case of UpdateVoxelMap per inserted point (lk_octree.cuh): a new root (1 node, one tile); per octree level one
+    // cut (8 nodes) whose children each get a tile — at most threshold + 1 of them hold a point when the cut fires; a
+    // tile is max_points_num + 2 slots (even). Reserving the bound makes a mid-insert overflow impossible: no point is
+    // ever dropped (the pools only grow when a scan could actually exceed them: 80 GB of HBM is the budget).
+    if (!rc) {
+        const Globals& g = h->g;
+        int thr = 0;
+        for (int l = 0; l < 5; ++l) thr = std::max(thr, g.layer_init_num[l]);
+        const uint64_t tile = (uint64_t)((g.max_points_num + 2 + 1) & ~1);
+        const uint64_t per_pt_nodes = 1 + 8ull * (uint64_t)std::max(g.max_layer, 0);
+        const uint64_t per_pt_slots = tile * (1 + (uint64_t)std::max(g.max_layer, 0) * (uint64_t)std::min(8, thr + 1)) + 2;
+        rc = h->map.ensure_headroom(n + 16, per_pt_nodes * n + 64, per_pt_slots * n + 64, s, h->err);
+    }
+    if (!rc) rc = h->map.push_counters(s, h->err);  // also makes what earlier launches freed available to this insert
+    if (rc) return rc;
+    if (h->ins_pend_nodes < h->map.node_cap) {
+        LK_CUDA(h->err, h->ins_pend.ensure((size_t)h->map.node_cap * 12));
+        LK_CUDA(h->err, cudaMemsetAsync(h->ins_pend.p, 0, h->ins_pend.cap, s));
+        h->ins_pend_nodes = h->map.node_cap;
+    }
+    return LK_OK;
+}
+
+// After the launches of an UpdateVoxelMap (fused: inside the per-scan kernel): wait for them, and report pools that ran
+// out (push_counters clears the flag).
+static int insert_finish(lk_handle h, bool fused) {
+    int rc = h->map.sync_counters(h->stream, h->err);  // also a sync
+    if (rc) return rc;
+    if (fused) {
+        rc = check_stall(h);
+        if (rc) return rc;
+    }
+    uint32_t ovf = 0;
+    LK_CUDA(h->err, cudaMemcpy(&ovf, h->map.dev().overflow, 4, cudaMemcpyDeviceToHost));
+    if (ovf) return fail(h, LK_ERR_CAPACITY, "map pools exhausted during UpdateVoxelMap (raise lk_map_reserve)");
+    return LK_OK;
+}
+
 // Enqueue the hot path for scans [first, first+count) of the staged batch; no host sync unless update_map.
 // timed: bracket the residual launches with events for lk_timer_stop.
 static int run_range_impl(lk_handle h, uint32_t first, uint32_t count, int iters, int update_map, const MeasQueue* mq,
@@ -1008,23 +1054,7 @@ static int run_range_impl(lk_handle h, uint32_t first, uint32_t count, int iters
     cudaStream_t s = h->stream;
     uint32_t max_bucket = 0;
     if (update_map) {
-        // UpdateVoxelMap may create the map: make room for this scan's points (roots, nodes, tiles)
-        const uint64_t n = h->h_scan_pts[first];
-        int rc = h->map.ready() ? h->map.sync_counters(s, h->err) : LK_OK;
-        // Worst case of UpdateVoxelMap per inserted point (lk_octree.cuh): a new root (1 node, one tile); per octree level one
-        // cut (8 nodes) whose children each get a tile — at most threshold + 1 of them hold a point when the cut fires; a
-        // tile is max_points_num + 2 slots (even). Reserving the bound makes a mid-insert overflow impossible: no point is
-        // ever dropped (the pools only grow when a scan could actually exceed them: 80 GB of HBM is the budget).
-        if (!rc) {
-            const Globals& g = h->g;
-            int thr = 0;
-            for (int l = 0; l < 5; ++l) thr = std::max(thr, g.layer_init_num[l]);
-            const uint64_t tile = (uint64_t)((g.max_points_num + 2 + 1) & ~1);
-            const uint64_t per_pt_nodes = 1 + 8ull * (uint64_t)std::max(g.max_layer, 0);
-            const uint64_t per_pt_slots = tile * (1 + (uint64_t)std::max(g.max_layer, 0) * (uint64_t)std::min(8, thr + 1)) + 2;
-            rc = h->map.ensure_headroom(n + 16, per_pt_nodes * n + 64, per_pt_slots * n + 64, s, h->err);
-        }
-        if (!rc) rc = h->map.push_counters(s, h->err);  // also makes what earlier launches freed available to this scan
+        int rc = insert_headroom(h, h->h_scan_pts[first]);
         if (rc) return rc;
         for (uint32_t k = 0; k < h->n_steps; ++k) {
             const StepInit& in = h->h_inits[(size_t)k * h->batch + first];
@@ -1037,11 +1067,6 @@ static int run_range_impl(lk_handle h, uint32_t first, uint32_t count, int iters
         LK_CUDA(h->err, h->ins_list.ensure(2 * mb * 4));
         LK_CUDA(h->err, h->ins_counters.ensure(64));
         LK_CUDA(h->err, cudaMemsetAsync(h->ins_counters.p, 0, 64, s));
-        if (h->ins_pend_nodes < h->map.node_cap) {
-            LK_CUDA(h->err, h->ins_pend.ensure((size_t)h->map.node_cap * 12));
-            LK_CUDA(h->err, cudaMemsetAsync(h->ins_pend.p, 0, h->ins_pend.cap, s));
-            h->ins_pend_nodes = h->map.node_cap;
-        }
     }
     if (!h->map.ready()) return fail(h, LK_ERR_NOT_READY, "no map: call lk_map_upload or lk_map_build first");
     // update_map inside the persistent kernel: buckets of up to 4 096 points (the root-per-point scan of its insert phase)
@@ -1055,15 +1080,93 @@ static int run_range_impl(lk_handle h, uint32_t first, uint32_t count, int iters
     if (rc || !update_map) return rc;
     // update_map: the caller observes a finished insert
     h->prev_fused = false;
-    rc = h->map.sync_counters(s, h->err);  // also a sync
-    if (rc) return rc;
-    if (fused) {
-        rc = check_stall(h);
-        if (rc) return rc;
+    return insert_finish(h, fused);
+}
+
+// lk_map_insert runs its input through the slice-and-sort insert in windows of at most this many points (DESIGN §3.5):
+// per window, the headroom a streaming scan of as many points reserves, and scratch of a fixed size.
+constexpr uint32_t MAP_INSERT_WINDOW = 32768u;
+
+int lk_map_insert(lk_handle h, uint32_t n_sets, const float* pts, const uint32_t* set_offsets, const double* rot,
+                  const double* pos, const double* rot_cov, const double* pos_cov) {
+    if (!h) return LK_ERR_INVALID_ARG;
+    if (n_sets == 0) return LK_OK;
+    if (!pts || !set_offsets || !rot || !pos || !rot_cov || !pos_cov) return fail(h, LK_ERR_INVALID_ARG, "null argument");
+    for (uint32_t s = 0; s < n_sets; ++s) {
+        if (set_offsets[s + 1] < set_offsets[s]) return fail(h, LK_ERR_INVALID_ARG, "set_offsets not monotone");
+        bool finite = true;
+        for (int i = 0; i < 9; ++i)
+            finite = finite && std::isfinite(rot[9 * (size_t)s + i]) && std::isfinite(rot_cov[9 * (size_t)s + i]) &&
+                     std::isfinite(pos_cov[9 * (size_t)s + i]);
+        for (int i = 0; i < 3; ++i) finite = finite && std::isfinite(pos[3 * (size_t)s + i]);
+        if (!finite) return fail(h, LK_ERR_INVALID_ARG, "non-finite pose or covariance");
     }
-    uint32_t ovf = 0;
-    LK_CUDA(h->err, cudaMemcpy(&ovf, h->map.dev().overflow, 4, cudaMemcpyDeviceToHost));
-    if (ovf) return fail(h, LK_ERR_CAPACITY, "map pools exhausted during UpdateVoxelMap (raise lk_map_reserve)");
+    enter(h);
+    cudaStream_t st = h->stream;
+    const uint32_t W = MAP_INSERT_WINDOW;
+    // a window holds points of at most W sets, and its chunks are 256 points each plus one partial chunk per set
+    const uint32_t max_sets = std::min(n_sets, W);
+    const size_t sc_off = align256(((size_t)W / 256u + max_sets) * sizeof(ChunkDesc));
+    const size_t small_bytes = sc_off + (size_t)max_sets * sizeof(ScanConst);
+    LK_CUDA(h->err, h->mi_pts.ensure((size_t)W * 16));
+    LK_CUDA(h->err, h->mi_ipts.ensure((size_t)W * insert_point_bytes()));
+    LK_CUDA(h->err, h->mi_root.ensure((size_t)W * 4));
+    LK_CUDA(h->err, h->mi_touched.ensure((size_t)W * 4));
+    LK_CUDA(h->err, h->mi_list.ensure((size_t)2 * W * 4));
+    LK_CUDA(h->err, h->mi_counters.ensure(64));
+    LK_CUDA(h->err, h->mi_small.ensure(small_bytes));
+    LK_CUDA(h->err, h->h_mi.ensure(small_bytes));
+    ChunkDesc* hc = reinterpret_cast<ChunkDesc*>(h->h_mi.p);
+    ScanConst* hs = reinterpret_cast<ScanConst*>((char*)h->h_mi.p + sc_off);
+    const ChunkDesc* dc = reinterpret_cast<const ChunkDesc*>(h->mi_small.p);
+    const ScanConst* ds = reinterpret_cast<const ScanConst*>((char*)h->mi_small.p + sc_off);
+    const uint64_t end = set_offsets[n_sets];
+    uint32_t s = 0;
+    for (uint64_t p0 = set_offsets[0]; p0 < end;) {
+        const uint64_t p1 = std::min<uint64_t>(end, p0 + W);
+        const uint32_t n = (uint32_t)(p1 - p0);
+        int rc = insert_headroom(h, n);
+        if (rc) return rc;
+        // the window's chunks; ChunkDesc.scan = the set's row in the window's table of placements
+        uint32_t nc = 0, nsc = 0;
+        while (set_offsets[s + 1] <= p0) ++s;
+        for (uint32_t t = s; t < n_sets && set_offsets[t] < p1; ++t) {
+            const uint64_t a = std::max<uint64_t>(set_offsets[t], p0), b = std::min<uint64_t>(set_offsets[t + 1], p1);
+            if (a >= b) continue;
+            // ScanConst as scan_const_from fills it from a filter: R, p and the symmetric parts of the two P blocks
+            ScanConst& sc = hs[nsc];
+            const double* R = rot + 9 * (size_t)t;
+            const double* Pt = rot_cov + 9 * (size_t)t;
+            const double* Pp = pos_cov + 9 * (size_t)t;
+            for (int i = 0; i < 9; ++i) sc.R[i] = R[i];
+            for (int i = 0; i < 3; ++i) sc.p[i] = pos[3 * (size_t)t + i];
+            const int ut[6][2] = {{0, 0}, {0, 1}, {0, 2}, {1, 1}, {1, 2}, {2, 2}};
+            for (int q = 0; q < 6; ++q) {
+                const int i = ut[q][0], j = ut[q][1];
+                sc.Pth[q] = 0.5 * (Pt[i * 3 + j] + Pt[j * 3 + i]);
+                sc.Ppp[q] = 0.5 * (Pp[i * 3 + j] + Pp[j * 3 + i]);
+            }
+            for (uint64_t q = a; q < b; q += 256) {
+                ChunkDesc& cd = hc[nc++];
+                cd.scan = nsc;
+                cd.start = (uint32_t)(q - p0);
+                cd.count = (uint32_t)std::min<uint64_t>(256, b - q);
+                cd.pad = 0;
+            }
+            ++nsc;
+        }
+        LK_CUDA(h->err, cudaMemcpyAsync(h->mi_pts.p, pts + 4 * p0, (size_t)n * 16, cudaMemcpyHostToDevice, st));
+        // (h_mi is free again: the previous window's insert_finish waited for its copies)
+        LK_CUDA(h->err, cudaMemcpyAsync(h->mi_small.p, hc, (size_t)nc * sizeof(ChunkDesc), cudaMemcpyHostToDevice, st));
+        LK_CUDA(h->err, cudaMemcpyAsync((char*)h->mi_small.p + sc_off, hs, (size_t)nsc * sizeof(ScanConst), cudaMemcpyHostToDevice, st));
+        map_insert_bucket(h->map, h->g, h->mi_pts.as<float4>(), dc, 0, nc, 0, n, ds, nullptr, h->mi_ipts.p,
+                          h->mi_root.as<int>(), h->ins_pend.as<int>(), h->mi_touched.as<uint32_t>(), h->mi_counters.as<uint32_t>(),
+                          h->mi_list.as<uint32_t>(), st);
+        LK_CUDA(h->err, cudaGetLastError());
+        rc = insert_finish(h, false);
+        if (rc) return rc;
+        p0 = p1;
+    }
     return LK_OK;
 }
 

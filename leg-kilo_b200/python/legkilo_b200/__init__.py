@@ -50,6 +50,7 @@ def lib():
         L.lk_map_upload.argtypes = [vp, vp, C.c_size_t]
         L.lk_map_download.argtypes = [vp, vp, C.c_size_t, vp]
         L.lk_map_build.argtypes = [vp, vp, vp, C.c_size_t, vp, vp, vp]
+        L.lk_map_insert.argtypes = [vp, u32, vp, vp, vp, vp, vp, vp]
         L.lk_map_stats.argtypes = [vp, vp]
         L.lk_map_slide.argtypes = [vp, vp, vp, vp]
         L.lk_map_memory.argtypes = [vp, vp]
@@ -179,6 +180,16 @@ class Engine:
         pos_cov = 1e-6 * np.eye(3) if pos_cov is None else np.ascontiguousarray(pos_cov, np.float64)
         self._chk(lib().lk_map_build(self.h, _p(xyz_world), _p(xyz_body), len(xyz_world), _p(R), _p(rot_cov),
                                      _p(pos_cov)))
+
+    def map_insert(self, pts, set_offsets, rot, pos, rot_cov, pos_cov):
+        """lk_map_insert: UpdateVoxelMap of point sets at known poses. pts float32 [n, 4] (lidar frame), set_offsets
+        [n_sets + 1]; per set rot [n_sets, 3, 3], pos [n_sets, 3], rot_cov / pos_cov [n_sets, 3, 3]."""
+        pts = np.ascontiguousarray(pts, np.float32).reshape(-1, 4)
+        so = np.ascontiguousarray(set_offsets, np.uint32)
+        n_sets = len(so) - 1
+        rot, pos, rot_cov, pos_cov = (np.ascontiguousarray(a, np.float64).reshape(n_sets, k)
+                                      for a, k in ((rot, 9), (pos, 3), (rot_cov, 9), (pos_cov, 9)))
+        self._chk(lib().lk_map_insert(self.h, n_sets, _p(pts), _p(so), _p(rot), _p(pos), _p(rot_cov), _p(pos_cov)))
 
     def map_slide(self, position):
         """VoxelMapManager::mapSliding (voxel_map.cc:552-571). Returns (slid, removed root voxels)."""
