@@ -112,6 +112,7 @@ struct lk_context {
     // direct mode of lk_scan_update (one scan, page-locked caller buffers): the kernel reads the points and
     // writes the world cloud / the filter in place, the small inputs ride in the kernel's parameter block
     int direct_io = 1, inline_in = 1, coop_launch = 0, pdl = 1, n_sms = 132, slim_p = 1;
+    int finishers = 1;  // per-scan kernel: run a single-bucket scan's epilogue on the SMs its chunks leave idle (lk_fused.cu)
     int fast_insert = 1;  // update_map: two-launch insert for small buckets, re-projection folded into it
     int fused_insert = 0;  // 1 = update_map of one scan with small buckets: UpdateVoxelMap inside the persistent kernel (one
                            // launch per scan; the serial per-root insert chain holds every other SM at the grid barrier)
@@ -419,7 +420,7 @@ int lk_set_param(lk_handle h, const char* name, double value) {
                  {"fused_insert", &lk_context::fused_insert},   {"coop_launch", &lk_context::coop_launch},
                  {"pdl", &lk_context::pdl},                     {"slim_p", &lk_context::slim_p},
                  {"direct_io", &lk_context::direct_io},         {"inline_in", &lk_context::inline_in},
-                 {"debug_records", &lk_context::debug_records}};
+                 {"debug_records", &lk_context::debug_records}, {"finishers", &lk_context::finishers}};
     for (const auto& k : knobs)
         if (!std::strcmp(name, k.name)) {
             h->*k.knob = (int)value;
@@ -827,6 +828,7 @@ static FusedArgs fused_args(lk_handle h, uint32_t first, int iters, bool insert,
     fa.ll.chunk_rows = h->ll.as<ulonglong2>();
     fa.ll.group_rows = h->ll.as<ulonglong2>() + (size_t)2 * LL_MAX_CHUNKS * LL_ROW;
     fa.ll.stall = reinterpret_cast<uint32_t*>((char*)h->ll.p + LL_ROWS_BYTES);
+    fa.ll.acks = reinterpret_cast<uint32_t*>((char*)h->ll.p + LL_ROWS_BYTES + 64);
     fa.epoch = h->ll_epoch;
     fa.iters = iters;
     fa.lane_cache = h->lane_cache;
@@ -848,6 +850,17 @@ static FusedArgs fused_args(lk_handle h, uint32_t first, int iters, bool insert,
         fa.n_meas = mq->n;
         fa.gravity = mq->gravity;
         fa.acc_norm = mq->acc_norm;
+    }
+    {
+        // finishers: one active bucket without a queue or insert, and SMs the chunks leave idle
+        const StepInit& in0 = h->h_inits[first];
+        const uint32_t sms = (uint32_t)fused_max_blocks(h->device), chunks = h->h_scan_chunks[first];
+        if (h->finishers && !insert && fa.n_meas == 0 && h->n_steps == 1 && in0.active && in0.chunk_end - in0.chunk_begin == chunks &&
+            chunks > 0 && iters >= 1 && chunks < sms) {  // the kernel's workers are then blocks [0, chunks)
+            fa.finishers = std::min(sms - chunks, (uint32_t)LL_MAX_FINISHERS);
+            // a finisher never reads host memory: in direct mode the workers copy their points to the staging buffer
+            if (h->direct) fa.pts_copy = h->pts.as<float4>();
+        }
     }
     fa.ecfg = h->ec;
     // back-to-back launches trace into consecutive areas (TRACE_AREA stamps each, TRACE_AREAS of them, cycling), so the
@@ -871,7 +884,6 @@ static FusedArgs fused_args(lk_handle h, uint32_t first, int iters, bool insert,
 // voxel to every warp of the grid.
 static int run_fused(lk_handle h, uint32_t first, int iters, bool insert, const MeasQueue* mq, bool timed) {
     cudaStream_t s = h->stream;
-    const uint32_t grid = insert ? (uint32_t)fused_max_blocks(h->device) : h->h_scan_chunks[first];
     FusedInline* inl = nullptr;
     if (h->inline_ok) {  // the staged filter and step table ride in the parameter block
         const char* hs = (const char*)h->h_small_in.p;
@@ -890,6 +902,7 @@ static int run_fused(lk_handle h, uint32_t first, int iters, bool insert, const 
         h->prev_fused = false;
     }
     const FusedArgs fa = fused_args(h, first, iters, insert, mq);
+    const uint32_t grid = insert ? (uint32_t)fused_max_blocks(h->device) : h->h_scan_chunks[first] + fa.finishers;
     h->ll_epoch += need;
     if (insert) h->prev_fused = false;  // the insert counters were cleared by a memset on the stream
     if (timed) { cudaEventRecord(kev_get(h, h->nev++), s); h->prev_fused = false; }

@@ -21,6 +21,12 @@
 // scan's blocks become resident and run their prologue (filter load, point prefetch) while this scan's
 // last blocks drain; everything that could collide with the previous launch (flagged rows, outputs) sits
 // behind griddepcontrol.wait.
+//
+// Finishers: a single-bucket launch without a queue or insert that leaves SMs idle gets up to LL_MAX_FINISHERS extra
+// blocks (FusedArgs::finishers). They follow every exchange and solve like the other blocks (their filter is the same),
+// but the chunk blocks — workers — leave at the last exchange as soon as their row is published: the last total, solve,
+// re-projection, covariance update and stores run on the finishers (fused_finish), while the workers' SMs already take
+// the next launch's blocks, which need none of that work until their own first exchange.
 #include "lk_insert.cuh"
 #include "lk_kernels.h"
 #include "lk_obs.cuh"
@@ -34,7 +40,8 @@ namespace {
 
 #define FT(slot) do { if (a.trace && threadIdx.x == 0 && (slot) < 32) a.trace[(size_t)blockIdx.x * 32 + (slot)] = gtime(); } while (0)
 // per-iteration stamps of the first three exchanges i: 14 + i pass done, 2 + 4i block row in shared memory, 3 + 4i all-reduce
-// total in shared memory, 4 + 4i solve done (tools/trace_fused.py)
+// total in shared memory, 4 + 4i solve done (tools/trace_fused.py); 23 / 24 before / after the first griddepcontrol.wait,
+// a finisher's 20 re-projection stored, 21 covariance stored, 22 state stored; 31 a block's end
 #define FTI(slot) do { if (it_global < 3) FT(slot); } while (0)
 // per-bucket stamps of the streaming variants (block 0, first 64 buckets, 8 stamps each, behind the per-block area)
 #define FTS(slot) do { if (a.trace && blockIdx.x == 0 && threadIdx.x == 0 && k < 64) a.trace[(size_t)gridDim.x * 32 + (size_t)k * 8 + (slot)] = gtime(); } while (0)
@@ -151,6 +158,81 @@ __device__ __noinline__ void fused_drain_queue(SM* sm, const FusedArgs& a, uint3
     }
 }
 
+// KILO.cc:216-224: a point of the world cloud at the updated state (pi: the point in the IMU frame, imu_point)
+__device__ __forceinline__ float4 world_out(const double* X, double pix, double piy, double piz, bool updated) {
+    float4 o;
+    o.x = (float)(X[0] * pix + X[1] * piy + X[2] * piz + X[9]);
+    o.y = (float)(X[3] * pix + X[4] * piy + X[5] * piz + X[10]);
+    o.z = (float)(X[6] * pix + X[7] * piy + X[8] * piz + X[11]);
+    o.w = updated ? 255.0f : 0.0f;
+    return o;
+}
+
+// The state, the clocks, the residual count and the status word of the scan (the covariance is stored by the caller).
+template <class SM>
+__device__ __forceinline__ void store_state(SM* sm, const FusedArgs& a, uint32_t n_eff) {
+    const int tid = threadIdx.x;
+    if (tid < 36) a.x[(size_t)a.scan * 36 + tid] = sm->f.x[tid];
+    if (tid < 2) reinterpret_cast<double*>(a.clk + a.scan)[tid] = sm->clk[tid];
+    if (tid == 0) {
+        a.n_eff[a.scan] = n_eff;
+        // did any wait of this launch give up (lk_llsync.cuh / lk_async.cuh watchdogs)? The host looks at this word first
+        // and only then pays for the detailed read-back
+        *a.status = (*reinterpret_cast<volatile uint32_t*>(a.ll.stall) ? 1u : 0u) | (*reinterpret_cast<volatile uint32_t*>(&lk_stall_note[0]) ? 2u : 0u);
+    }
+}
+
+// The epilogue of a launch with finishers, run by each finisher (blocks n_chunks .. gridDim.x - 1) at the scan's last
+// exchange: that exchange in one hop from the chunk rows, the last solve, then the re-projection and the covariance update
+// split over the finishers, and the stores. The workers have left by then; the filter they would have ended with is the
+// one every finisher holds. Out of line, so the workers' register allocation is that of the kernel without it.
+template <class SM>
+__device__ __noinline__ void fused_finish(SM* sm, const FusedArgs& a, const StepInit& in, uint32_t n_chunks, uint32_t it_global,
+                                          bool updated, bool dep_waited) {
+    const int tid = threadIdx.x;
+    const uint32_t fi = blockIdx.x - n_chunks, nf = gridDim.x - n_chunks;
+    if (!dep_waited) asm volatile("griddepcontrol.wait;" ::: "memory");  // the rows / outputs of the previous launch
+    ll_sum_chunk_rows<WARPS>(a.ll, it_global & 1u, a.epoch + it_global, n_chunks, sm->u.pr.F, sm->f.acc);
+    FTI(3 + it_global * 4);
+    const uint32_t n = block_solve_state(&sm->f);
+    FTI(4 + it_global * 4);
+    if (n > 0) {
+        updated = true;
+        if (tid == 0) sm->clk[1] = in.t_bucket;  // KILO.cc:212
+    }
+    // re-projection (KILO.cc:216-224). Direct mode: from the workers' device copy of the points, stored before their last
+    // row (the fence makes those stores visible here); the points are never read from host memory by a finisher.
+    const float4* pts = a.pts;
+    if (a.pts_copy) {
+        __threadfence();
+        pts = a.pts_copy;
+    }
+    // a thread's points in batches of U, all loads of a batch issued before the first store (one L2 round trip per batch)
+    constexpr int U = 8;
+    const uint32_t step = nf * BLOCK;
+    for (uint32_t i0 = in.pt_begin + fi * BLOCK + tid; i0 < in.pt_end; i0 += U * step) {
+        float4 q[U];
+#pragma unroll
+        for (int u = 0; u < U; ++u)
+            if (i0 + u * step < in.pt_end) q[u] = __ldcg(pts + i0 + u * step);
+#pragma unroll
+        for (int u = 0; u < U; ++u)
+            if (i0 + u * step < in.pt_end) {
+                PointCtx p;
+                imu_point(q[u], a.g, p);
+                a.world[i0 + u * step] = world_out(sm->f.x, p.pix, p.piy, p.piz, updated);
+            }
+    }
+    FT(20);
+    if (n > 0) cov_prep(&sm->f, BLOCK);
+    __syncthreads();
+    for (uint32_t e = fi * BLOCK + tid; e < 900; e += nf * BLOCK)
+        a.P[(size_t)a.scan * 900 + e] = n > 0 ? cov_entry(&sm->f, (int)e) : sm->f.P[e];
+    FT(21);
+    if (fi == 0) store_state(sm, a, n);
+    FT(22);
+}
+
 template <bool INL> struct InlineSel { typedef FusedInline type; };
 template <> struct InlineSel<false> { typedef FusedNoInline type; };
 
@@ -179,6 +261,8 @@ __global__ void __launch_bounds__(BLOCK, 1) k_scan_fused(const __grid_constant__
     FusedSmemT<!INS>* sm = reinterpret_cast<FusedSmemT<!INS>*>(smem_raw);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const uint32_t scan = a.scan;
+    // a.finishers > 0: the last a.finishers blocks of the grid are finishers (fused_finish), the others workers
+    const bool finisher = blockIdx.x + a.finishers >= gridDim.x;
     // let the next launch of the stream (if it was launched with programmatic serialisation) start placing its
     // blocks as soon as this grid's blocks are all running; it blocks in griddepcontrol.wait until we are done
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
@@ -190,9 +274,10 @@ __global__ void __launch_bounds__(BLOCK, 1) k_scan_fused(const __grid_constant__
         const double* cin;
         if constexpr (INL) { Pin = inl.P; xin = inl.x; cin = inl.clk; }
         else { Pin = a.P_in + (size_t)scan * 900; xin = a.x_in + (size_t)scan * 36; cin = reinterpret_cast<const double*>(a.clk_in + scan); }
-        if (a.slim_p && blockIdx.x != 0) {
-            // a single-bucket scan without a queue never predicts; blocks other than 0 (which stores the covariance) then
-            // only ever read P[:, 0:6]: the 6x6 corner for the solve and the scan constants, the 30x6 strip for delta
+        if (a.slim_p && !finisher && (a.finishers || blockIdx.x != 0)) {
+            // a single-bucket scan without a queue never predicts; blocks that do not store the covariance (all but block
+            // 0, or all workers) then only ever read P[:, 0:6]: the 6x6 corner for the solve and the scan constants, the
+            // 30x6 strip for delta
             if (tid < 180) sm->f.P[(tid / 6) * 30 + tid % 6] = Pin[(tid / 6) * 30 + tid % 6];
         } else {
             for (int e = tid; e < 900; e += BLOCK) sm->f.P[e] = Pin[e];
@@ -260,13 +345,41 @@ __global__ void __launch_bounds__(BLOCK, 1) k_scan_fused(const __grid_constant__
             __syncthreads();
             FTI(2 + it_global * 4);
             if (it == 0) FTS(3);
+            const bool last = it == a.iters - 1;
+            if (!OBS && !INS && a.finishers && last) {
+                // the last exchange of a launch with finishers (a single bucket): a worker publishes its row and leaves, the
+                // finishers take it from there; the SMs of the workers go to the next launch
+                if (finisher) {
+                    fused_finish(sm, a, in, n_chunks, it_global, updated, dep_waited);
+                } else {
+                    if (!dep_waited) asm volatile("griddepcontrol.wait;" ::: "memory");  // the rows of the previous launch
+                    if (a.pts_copy) {  // direct mode: the finishers re-project from a device copy (fused_finish)
+                        if ((uint32_t)tid < my_count) a.pts_copy[my_start + tid] = pre;
+                        __threadfence();
+                        __syncthreads();
+                    }
+                    if (warp == 0) {
+                        double v = 0.0;
+#pragma unroll
+                        for (int w = 0; w < WARPS; ++w) v += sm->slice[w * 32 + lane];
+                        ll_publish_row(a.ll, it_global & 1u, a.epoch + it_global, blockIdx.x, v, lane);
+                    }
+                }
+                FT(31);
+                return;
+            }
             // 2) all-reduce of the block rows (warp 0), no barrier
             if (warp == 0) {
                 double v = 0.0;
 #pragma unroll
                 for (int w = 0; w < WARPS; ++w) v += sm->slice[w * 32 + lane];
-                if (!dep_waited) asm volatile("griddepcontrol.wait;" ::: "memory");  // the rows / outputs of the previous launch
-                sm->f.acc[lane] = ll_allreduce(a.ll, it_global & 1u, a.epoch + it_global, blockIdx.x, n_chunks, v, lane, FT_HOPS());
+                if (!dep_waited) {  // the rows / outputs of the previous launch
+                    FT(23);
+                    asm volatile("griddepcontrol.wait;" ::: "memory");
+                    FT(24);
+                }
+                sm->f.acc[lane] = ll_allreduce(a.ll, it_global & 1u, a.epoch + it_global, blockIdx.x, n_chunks, v, lane, FT_HOPS(),
+                                               a.finishers, it_global >= 2);
             }
             dep_waited = true;
             __syncthreads();
@@ -274,7 +387,6 @@ __global__ void __launch_bounds__(BLOCK, 1) k_scan_fused(const __grid_constant__
             if (it == 0) FTS(4);
             // 3) every block solves redundantly (eskf.cc:91-113); the covariance update of the last iteration is
             //    deferred behind the re-projection, and skipped where nobody reads the result
-            const bool last = it == a.iters - 1;
             const uint32_t n = block_solve_state(&sm->f);
             FTI(4 + it_global * 4);
             if (n > 0) {
@@ -288,15 +400,7 @@ __global__ void __launch_bounds__(BLOCK, 1) k_scan_fused(const __grid_constant__
         FTS(5);
         if constexpr (!INS) {
             // 4) re-projection with the updated state (KILO.cc:216-224)
-            if ((uint32_t)tid < my_count) {
-                const double* X = sm->f.x;
-                float4 o;
-                o.x = (float)(X[0] * lc.pix + X[1] * lc.piy + X[2] * lc.piz + X[9]);
-                o.y = (float)(X[3] * lc.pix + X[4] * lc.piy + X[5] * lc.piz + X[10]);
-                o.z = (float)(X[6] * lc.pix + X[7] * lc.piy + X[8] * lc.piz + X[11]);
-                o.w = updated ? 255.0f : 0.0f;
-                a.world[my_start + tid] = o;
-            }
+            if ((uint32_t)tid < my_count) a.world[my_start + tid] = world_out(sm->f.x, lc.pix, lc.piy, lc.piz, updated);
             FT(20);
             if (cov_pending) block_cov_update<BLOCK>(&sm->f);
         } else {
@@ -339,14 +443,7 @@ __global__ void __launch_bounds__(BLOCK, 1) k_scan_fused(const __grid_constant__
         if (!dep_waited) asm volatile("griddepcontrol.wait;" ::: "memory");
         __syncthreads();
         for (int e = tid; e < 900; e += BLOCK) a.P[(size_t)scan * 900 + e] = sm->f.P[e];
-        if (tid < 36) a.x[(size_t)scan * 36 + tid] = sm->f.x[tid];
-        if (tid < 2) reinterpret_cast<double*>(a.clk + scan)[tid] = sm->clk[tid];
-        if (tid == 0) {
-            a.n_eff[scan] = n_eff_total;
-            // did any wait of this launch give up (lk_llsync.cuh / lk_async.cuh watchdogs)? The host looks at this word first
-            // and only then pays for the detailed read-back
-            *a.status = (*reinterpret_cast<volatile uint32_t*>(a.ll.stall) ? 1u : 0u) | (*reinterpret_cast<volatile uint32_t*>(&lk_stall_note[0]) ? 2u : 0u);
-        }
+        store_state(sm, a, n_eff_total);
     }
     FT(31);
 }

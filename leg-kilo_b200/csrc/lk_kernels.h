@@ -137,6 +137,10 @@ struct FusedArgs {
     int iters;
     int lane_cache;  // keep per-lane lookups / staged records across the iterations of a bucket
     int slim_p;        // blocks other than 0 load only P[:, 0:6] (valid when the scan has one bucket, no queue, no predict)
+    // > 0 (one active bucket, no queue, no insert): the last `finishers` blocks of the grid run the scan's epilogue and the
+    // others leave at their last row (lk_fused.cu)
+    uint32_t finishers;
+    float4* pts_copy;  // with finishers and points in host memory: device copy of the points the workers make for them
     MapView mv;
     const lk_imu_meas* imu;      // queued samples interleaved with the buckets (exactly one of imu / kin, or none)
     const lk_kinimu_meas* kin;

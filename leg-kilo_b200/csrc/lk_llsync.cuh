@@ -18,6 +18,13 @@
 // there, so the chain does not order its reads of i before the writes of i+2; it only holds because such a
 // block would have to lag a whole pass and solve behind the others. This is as old as the two buffers.
 //
+// Finishers (lk_fused.cu) are such blocks, made safe by construction: they read a copy of the group rows of
+// their own (copy LL_REPLICAS, written only when the launch has finishers) and, after reading exchange i,
+// store an acknowledgement word tagged i; a leader of exchange i+2 polls those words before it writes its
+// group row. A finisher takes the LAST exchange of its launch straight from the chunk rows (ll_sum_chunk_rows),
+// which every block then publishes, leaders included; nothing writes rows after it within the launch, and the
+// next launch writes rows only behind griddepcontrol.wait.
+//
 // Summation order (shared with the multi-kernel path, lk_solve.cuh: block_sum_partials):
 //   total = sum over groups g ascending of ( sum over the rows of group g ascending ),
 //   group g = chunks [g*LK_GROUP, (g+1)*LK_GROUP) of the bucket — a function of the bucket alone.
@@ -34,14 +41,17 @@ constexpr int LL_ROW = 32;           // slots (doubles) per row
 constexpr int LL_MAX_CHUNKS = 160;   // >= SM count: the fused kernel runs one chunk per block
 constexpr int LL_MAX_GROUPS = (LL_MAX_CHUNKS + LK_GROUP - 1) / LK_GROUP;
 constexpr int LL_REPLICAS = 4;       // copies of every group row (level-2 readers per copy: blocks / LL_REPLICAS)
+constexpr int LL_COPIES = LL_REPLICAS + 1;  // + the finishers' copy
+constexpr int LL_MAX_FINISHERS = 24;  // one acknowledgement word per finisher, polled one per lane
 
 struct LLView {
     ulonglong2* chunk_rows;  // [2][LL_MAX_CHUNKS][LL_ROW]
-    ulonglong2* group_rows;  // [2][LL_REPLICAS][LL_MAX_GROUPS][LL_ROW]
+    ulonglong2* group_rows;  // [2][LL_COPIES][LL_MAX_GROUPS][LL_ROW]
     uint32_t* stall;         // [8] watchdog record: [0] != 0 once a poll gave up | block | tag | first row | rows | lane
+    uint32_t* acks;          // [2][LL_MAX_FINISHERS] tag of the last exchange each finisher has read
 };
-constexpr size_t LL_ROWS_BYTES = (size_t)2 * (LL_MAX_CHUNKS + LL_REPLICAS * LL_MAX_GROUPS) * LL_ROW * sizeof(ulonglong2);
-constexpr size_t LL_BYTES = LL_ROWS_BYTES + 64;
+constexpr size_t LL_ROWS_BYTES = (size_t)2 * (LL_MAX_CHUNKS + LL_COPIES * LL_MAX_GROUPS) * LL_ROW * sizeof(ulonglong2);
+constexpr size_t LL_BYTES = LL_ROWS_BYTES + 64 + 2 * LL_MAX_FINISHERS * sizeof(uint32_t);
 // A poll that sees nothing for this many rounds (seconds) gives up, records who waited for what and lets the kernel run
 // to its end with garbage sums; the host then reports LK_ERR_CUDA instead of hanging. It means the blocks of the grid were
 // not all resident (another process holds SMs: see INTEGRATION.md "Sharing a device") — or a bug.
@@ -132,16 +142,38 @@ __device__ __forceinline__ double ll_sum_rows(const ulonglong2* rows, uint32_t r
     return s;
 }
 
+// Waits until finishers [0, fin) have acknowledged exchange `tag` (a group leader, before it rewrites the buffers that
+// exchange used). One full warp, fin <= 32.
+__device__ __forceinline__ void ll_wait_acks(const uint32_t* acks, uint32_t fin, uint32_t tag, int lane, uint32_t* stall) {
+    uint32_t spins = 0;
+    bool mine = (uint32_t)lane >= fin;
+    while (!__all_sync(0xffffffffu, mine)) {
+        if (!mine) {
+            uint32_t w;
+            asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(w) : "l"(acks + lane) : "memory");
+            mine = w == tag;
+        }
+        if ((++spins & 0xfffu) == 0u && (spins >= LL_SPIN_LIMIT || *reinterpret_cast<volatile uint32_t*>(stall) != 0u)) {
+            ll_give_up(stall, tag, 0, fin, lane);
+            break;
+        }
+    }
+}
+
 // The all-reduce. `v` = this block's row element `lane` (warp 0 calls, all 32 lanes). Block b owns
 // chunk b of the n_chunks chunks of the bucket (blocks with b >= n_chunks contribute nothing but still receive the
 // total). Returns the total of element `lane` in the fixed grouped order. Level 1: rows travel through global memory in
 // the flagged format, the group's first block adds them; level 2: it publishes the group row in LL_REPLICAS copies, every
 // block polls its copy of the (<= 20) group rows. `hops` (nullptr: no trace) receives LL_HOP_SLOTS stamps and counts.
+// `fin` > 0: the launch has `fin` finishers, blocks n_chunks .. n_chunks + fin - 1; leaders also write the finishers'
+// copy, and when `acks_due` (exchange tag - 2 is of this launch) first wait for every finisher to have read it.
 __device__ __forceinline__ double ll_allreduce(const LLView& ll, uint32_t parity, uint32_t tag, uint32_t b, uint32_t n_chunks,
-                                               double v, int lane, unsigned long long* hops = nullptr) {
+                                               double v, int lane, unsigned long long* hops = nullptr, uint32_t fin = 0,
+                                               bool acks_due = false) {
     constexpr size_t COPY = (size_t)LL_MAX_GROUPS * LL_ROW;
     ulonglong2* crows = ll.chunk_rows + (size_t)parity * LL_MAX_CHUNKS * LL_ROW;
-    ulonglong2* grows = ll.group_rows + (size_t)parity * LL_REPLICAS * COPY;
+    ulonglong2* grows = ll.group_rows + (size_t)parity * LL_COPIES * COPY;
+    uint32_t* acks = ll.acks + (size_t)parity * LL_MAX_FINISHERS;
     const uint32_t n_groups = (n_chunks + LK_GROUP - 1) / LK_GROUP;
     uint32_t r1 = 0, r2 = 0;
     if (b < n_chunks) {
@@ -151,15 +183,23 @@ __device__ __forceinline__ double ll_allreduce(const LLView& ll, uint32_t parity
             const double s = ll_sum_rows<LK_GROUP, false>(crows, b, n, tag, lane, ll.stall, r1, v, true);
             if (hops && lane == 0) hops[1] = gtime();
             ulonglong2* g = grows + (size_t)(b / LK_GROUP) * LL_ROW + lane;
+            if (fin && acks_due) ll_wait_acks(acks, fin, tag - 2u, lane, ll.stall);
 #pragma unroll
             for (int r = 0; r < LL_REPLICAS; ++r) ll_store(g + (size_t)r * COPY, s, tag);
+            if (fin) ll_store(g + (size_t)LL_REPLICAS * COPY, s, tag);
             if (hops && lane == 0) hops[2] = gtime();
         } else {
             ll_store(crows + (size_t)b * LL_ROW + lane, v, tag);
             if (hops && lane == 0) hops[0] = gtime();
         }
     }
-    const double t = ll_sum_rows<LL_MAX_GROUPS, true>(grows + (size_t)(b % LL_REPLICAS) * COPY, 0, n_groups, tag, lane, ll.stall, r2);
+    const bool finisher = fin && b >= n_chunks;
+    const double t = ll_sum_rows<LL_MAX_GROUPS, true>(grows + (size_t)(finisher ? LL_REPLICAS : b % LL_REPLICAS) * COPY, 0, n_groups,
+                                                      tag, lane, ll.stall, r2);
+    if (finisher) {  // every lane's reads of this exchange are done before the word says so
+        __syncwarp();
+        if (lane == 0) asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(acks + (b - n_chunks)), "r"(tag) : "memory");
+    }
     if (hops) {
         r1 = __reduce_max_sync(0xffffffffu, r1);
         r2 = __reduce_max_sync(0xffffffffu, r2);
@@ -169,6 +209,36 @@ __device__ __forceinline__ double ll_allreduce(const LLView& ll, uint32_t parity
         }
     }
     return t;
+}
+
+// The last exchange of a launch with finishers, the worker side: block b < n_chunks publishes its chunk row (a leader
+// too) and is done with the exchange. Warp 0 calls, all 32 lanes.
+__device__ __forceinline__ void ll_publish_row(const LLView& ll, uint32_t parity, uint32_t tag, uint32_t b, double v, int lane) {
+    ll_store(ll.chunk_rows + ((size_t)parity * LL_MAX_CHUNKS + b) * LL_ROW + lane, v, tag);
+}
+
+// The last exchange of a launch with finishers, the finisher side: the total of the n_chunks chunk rows in one hop, in
+// the grouped order of ll_allreduce (each group summed from 0.0 in ascending row order, then the group sums in ascending
+// order). Warp w sums groups w, w + NWARPS, ... into gs[g * 32 + lane] (LL_MAX_GROUPS * 32 doubles); result in
+// out[0..31]. All threads of the block call.
+template <int NWARPS>
+__device__ __forceinline__ void ll_sum_chunk_rows(const LLView& ll, uint32_t parity, uint32_t tag, uint32_t n_chunks, double* gs,
+                                                  double* out) {
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const ulonglong2* crows = ll.chunk_rows + (size_t)parity * LL_MAX_CHUNKS * LL_ROW;
+    const uint32_t n_groups = (n_chunks + LK_GROUP - 1) / LK_GROUP;
+    for (uint32_t g = (uint32_t)warp; g < n_groups; g += NWARPS) {
+        uint32_t rounds;
+        gs[g * 32 + lane] = ll_sum_rows<LK_GROUP, false>(crows, g * LK_GROUP, min((uint32_t)LK_GROUP, n_chunks - g * LK_GROUP), tag,
+                                                         lane, ll.stall, rounds);
+    }
+    __syncthreads();
+    if (tid < 32) {
+        double t = 0.0;
+        for (uint32_t g = 0; g < n_groups; ++g) t += gs[g * 32 + tid];
+        out[tid] = t;
+    }
+    __syncthreads();
 }
 
 }  // namespace lk

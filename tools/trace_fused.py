@@ -8,7 +8,10 @@ overlap through programmatic dependent launch). Only those launches carry stamps
 first of them follows the switch that turns tracing on and is launched without PDL, so it is left out of the figures.
 Stamps per block (slots, see lk_fused.cu): 0 entry, 1 first pass starts, per iteration i 14+i pass done,
 2+4i block row in shared memory, 3+4i all-reduce total in hand, 4+4i solve done, 20 re-projection stored, 30 loop left,
-31 end; a build without the pass-done and re-projection stamps gets the combined phases printed instead. Times in
+31 end, 23 / 24 around the first griddepcontrol.wait; a build without the pass-done and re-projection stamps gets the
+combined phases printed instead. With finishers (lk_set_param "finishers", on by default) the launch has extra blocks
+behind the chunk blocks (workers), which leave at their last row: the finishers' phases of the last exchange (total in
+hand, solve, re-projection 20, covariance 21, state stores 22) are printed against the last worker row. Times in
 microseconds: medians over the traced launches (min and max beside them) of per-launch medians over blocks, unless the
 name says "slowest block" or "last block".
 
@@ -33,7 +36,7 @@ import legkilo_b200  # noqa: E402
 from legkilo_b200 import Engine, _p, abi, lib  # noqa: E402
 
 TRACE_AREA, TRACE_AREAS = 8192, 64  # lk_api.cu
-HOP_SLOTS, GROUP = 5, 8  # lk_llsync.cuh: LL_HOP_SLOTS, LK_GROUP
+HOP_SLOTS, GROUP, MAX_FINISHERS = 5, 8, 24  # lk_llsync.cuh: LL_HOP_SLOTS, LK_GROUP, LL_MAX_FINISHERS
 
 
 def main():
@@ -74,12 +77,18 @@ def main():
     eng.set_param("trace", 0)
     offs = wl["offs"]
     T = []
+    NB = []
     H = [] if args.hops else None
+    fin_on = dict(kv.split("=") for kv in args.param).get("finishers", "1") != "0"
+    import torch
+    sms = min(torch.cuda.get_device_properties(0).multi_processor_count, 160)  # lk_fused.cu: fused_max_blocks
     for j, s in enumerate(scans):
         nb = int((offs[s + 1] - offs[s] + 255) // 256)
-        T.append(tr[j * TRACE_AREA: j * TRACE_AREA + nb * 32].reshape(nb, 32).astype(np.int64))
+        grid = nb + (min(sms - nb, MAX_FINISHERS) if fin_on and nb < sms else 0)  # lk_api.cu: fused_args
+        NB.append(nb)
+        T.append(tr[j * TRACE_AREA: j * TRACE_AREA + grid * 32].reshape(grid, 32).astype(np.int64))
         if args.hops:
-            h0 = j * TRACE_AREA + nb * 32 + 64 * 8
+            h0 = j * TRACE_AREA + grid * 32 + 64 * 8
             H.append(tr[h0: h0 + nb * 16].reshape(nb, 16).astype(np.int64))
     if args.hops and not any(h.any() for h in H):
         sys.exit("%s wrote no hop stamps: it was built without LK_HOP_TRACE" % legkilo_b200.LIB_PATH)
@@ -95,12 +104,32 @@ def main():
         rows.setdefault(name, []).append(v)
 
     for j in range(1, L):
-        b = T[j]
-        t0 = b[:, 0].min()
+        nb = NB[j]
+        fin = T[j][nb:]  # finishers (none without them)
+        b = T[j][:nb]    # workers: the chunk blocks
+        t0 = T[j][:, 0].min()
         put("launch: block start spread", (b[:, 0].max() - t0) * us)
         put("prologue (entry -> first pass)", np.median(b[:, 1] - b[:, 0]) * us)
         prev = b[:, 1]
+        if has(b, 24):
+            put("first griddepcontrol.wait: blocked (median block)", np.median(b[:, 24] - b[:, 23]) * us)
+            put("first griddepcontrol.wait: blocked (most)", (b[:, 24] - b[:, 23]).max() * us)
         for it in range(it_n):
+            s_row, s_ar, s_sol, s_pass = 2 + 4 * it, 3 + 4 * it, 4 + 4 * it, 14 + it
+            if len(fin) and it == it_n - 1:  # the workers leave at their last row; the finishers take it from there
+                if has(b, s_pass):
+                    put("it%d pass" % it, np.median(b[:, s_pass] - prev) * us)
+                put("it%d pass + reduction: slowest worker" % it, (b[:, s_row] - prev).max() * us)
+                last_in = b[:, s_row].max()
+                put("it%d workers: last row -> last worker end" % it, (b[:, 31].max() - last_in) * us)
+                put("finishers: last row -> total in hand (median)", (np.median(fin[:, s_ar]) - last_in) * us)
+                put("finishers: solve", np.median(fin[:, s_sol] - fin[:, s_ar]) * us)
+                put("finishers: re-projection", np.median(fin[:, 20] - fin[:, s_sol]) * us)
+                put("finishers: covariance", np.median(fin[:, 21] - fin[:, 20]) * us)
+                put("finishers: state stores (finisher 0)", (fin[0, 22] - fin[0, 21]) * us)
+                put("finishers: last row -> last finisher end", (fin[:, 31].max() - last_in) * us)
+                put("finishers: start after first worker start (median)", (np.median(fin[:, 0]) - b[:, 0].min()) * us)
+                break
             s_row, s_ar, s_sol, s_pass = 2 + 4 * it, 3 + 4 * it, 4 + 4 * it, 14 + it
             if has(b, s_pass):
                 put("it%d pass" % it, np.median(b[:, s_pass] - prev) * us)
@@ -126,18 +155,20 @@ def main():
                 put("it%d poll rounds hop 1 (most)" % it, (h[lead, 4] & 0xffffffff).max())
                 put("it%d poll rounds hop 2 (median block)" % it, np.median(h[:, 4] >> 32))
                 put("it%d poll rounds hop 2 (most)" % it, (h[:, 4] >> 32).max())
-        if has(b, 20):
-            put("re-projection", np.median(b[:, 20] - prev) * us)
-            put("after re-projection -> loop left", np.median(b[:, 30] - b[:, 20]) * us)
-        else:
-            put("re-projection (+ cov)", np.median(b[:, 30] - prev) * us)
-        put("block 0 tail (cov update, P store)", (b[0, 31] - b[0, 30]) * us)
-        put("launch span (first entry -> last end)", (b[:, 31].max() - t0) * us)
+        if not len(fin):
+            if has(b, 20):
+                put("re-projection", np.median(b[:, 20] - prev) * us)
+                put("after re-projection -> loop left", np.median(b[:, 30] - b[:, 20]) * us)
+            else:
+                put("re-projection (+ cov)", np.median(b[:, 30] - prev) * us)
+            put("block 0 tail (cov update, P store)", (b[0, 31] - b[0, 30]) * us)
+        end = T[j][:, 31].max()
+        put("launch span (first entry -> last end)", (end - t0) * us)
         if j + 1 < L:
-            n = T[j + 1]
-            put("next launch: first block entry - this launch's last end", (n[:, 0].min() - b[:, 31].max()) * us)
-            put("next launch: first exchange done - this launch's last end", (n[:, 3].min() - b[:, 31].max()) * us)
-            put("period (first entry to next first entry)", (n[:, 0].min() - t0) * us)
+            n = T[j + 1][:NB[j + 1]]
+            put("next launch: first block entry - this launch's last end", (n[:, 0].min() - end) * us)
+            put("next launch: first exchange done - this launch's last end", (n[:, 3].min() - end) * us)
+            put("period (first entry to next first entry)", (T[j + 1][:, 0].min() - t0) * us)
     nbs = sorted({t.shape[0] for t in T})
     print("%s, ring %d, %d traced launches (%d..%d blocks), %s" % (args.workload, ring, L - 1, nbs[0], nbs[-1], bench.gpu_identity(0)))
     for k, v in rows.items():
