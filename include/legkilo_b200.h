@@ -385,6 +385,23 @@ int lk_decode_pointcloud2(lk_handle h, const uint8_t* data, uint32_t n_points, c
 int lk_preprocess_scan(lk_handle h, const float* pts_in, uint32_t n_in, float leaf_size, float* pts_out,
                        uint32_t* n_out, uint32_t* bucket_offsets, float* bucket_curvature, uint32_t* n_buckets);
 
+/* lk_preprocess_scan for n_scans scans in one call, output in the layout lk_batch_stage / lk_scan_update take.
+ * Scan s is pts_in[in_offsets[s] .. in_offsets[s+1]) (float4 x, y, z, curvature). Every scan is filtered with leaf_size
+ * on its OWN bounding box (PCL 1.8 semantics, as lk_preprocess_scan), then stable-sorted by curvature and cut into maximal
+ * equal-curvature runs; each scan's output is bitwise what lk_preprocess_scan gives for it alone.
+ * Out (capacities from N = in_offsets[n_scans]): pts_out N float4; scan_offsets / scan_bucket_ptr n_scans + 1;
+ * bucket_offsets N + 1 (global point indices); bucket_curvature N; bucket_times N, written iff begin_times != NULL:
+ * bucket_times[b] = begin_times[s] + (double)bucket_curvature[b] (KILO.cc:376). Totals are scan_offsets[n_scans] and
+ * scan_bucket_ptr[n_scans]. A scan with no finite point yields zero points and zero buckets.
+ * LK_ERR_INVALID_ARG: a NULL argument, in_offsets not monotone, leaf_size not positive and finite, begin_times given
+ * without bucket_times or the reverse, or a scan whose leaf index would overflow int32 (lk_last_error names the scan;
+ * nothing is written). n_scans == 0 writes scan_offsets[0] = scan_bucket_ptr[0] = bucket_offsets[0] = 0.
+ * Runs on the device with a fixed number of host synchronisations (four) whatever n_scans is; its device memory is kept
+ * by the handle and grown to the largest call. */
+int lk_preprocess_scans(lk_handle h, uint32_t n_scans, const float* pts_in, const uint32_t* in_offsets, float leaf_size,
+                        const double* begin_times, float* pts_out, uint32_t* scan_offsets, uint32_t* scan_bucket_ptr,
+                        uint32_t* bucket_offsets, float* bucket_curvature, double* bucket_times);
+
 /* ---- leg kinematics: what feeds lk_obs_kinimu / the kin queue of lk_process_scan ----------- */
 
 /* = legkilo::Kinematics::Config (kinematics.h:27-35), same field order. */

@@ -16,9 +16,9 @@ namespace lk {
 int decode_pointcloud2_device(const uint8_t* h_data, uint32_t n, const lk_pc2_layout& L, float blind, int filter_num,
                               double time_scale, float* h_pts_out, float* h_intensity_out, uint32_t* n_out, cudaStream_t s,
                               std::string& err);
-int preprocess_scan_device(const float* h_pts_in, uint32_t n, float leaf, float* h_pts_out, uint32_t* n_out,
-                           uint32_t* h_bucket_offsets, float* h_bucket_curv, uint32_t* n_buckets, cudaStream_t s,
-                           std::string& err);
+int preprocess_scans_device(uint32_t n_scans, const float* h_pts_in, const uint32_t* h_offs, float leaf, const double* h_begin,
+                            float* h_pts_out, uint32_t* h_scan_off, uint32_t* h_scan_bptr, uint32_t* h_boff, float* h_bcurv,
+                            double* h_btimes, DevBuf& scratch, cudaStream_t s, std::string& err);
 size_t leg_kinematics_scratch_bytes(uint32_t n);
 int leg_kinematics_device(const lk_leg_cfg& cfg, const lk_leg_state* h_in, uint32_t n, int redundancy,
                           lk_leg_track* track, lk_kinimu_meas* h_out, uint32_t* n_out, void* scratch, cudaStream_t s,
@@ -123,6 +123,7 @@ struct lk_context {
     double hprof[8] = {0, 0, 0, 0, 0, 0, 0, 0};  // host-side ns of lk_scan_update: stage | enqueue | wait+fetch | calls
     DevBuf Qc;                     // process noise kept on the device between calls
     DevBuf leg_scratch;            // lk_leg_kinematics: inputs, flags, scans and outputs of the last call's size
+    DevBuf pre_scratch;            // lk_preprocess_scan(s): points, keys, leaves and buckets of the largest call
     std::vector<double> Q_shadow;  // what Qc holds
 
     // timing
@@ -1472,9 +1473,35 @@ int lk_preprocess_scan(lk_handle h, const float* pts_in, uint32_t n_in, float le
     if (!h || !n_out || !n_buckets || !bucket_offsets || (n_in && (!pts_in || !pts_out || !bucket_curvature)))
         return fail(h, LK_ERR_INVALID_ARG, "null argument");
     if (!(leaf_size > 0)) return fail(h, LK_ERR_INVALID_ARG, "leaf size must be positive");
+    *n_out = 0;
+    *n_buckets = 0;
     enter(h);
-    return preprocess_scan_device(pts_in, n_in, leaf_size, pts_out, n_out, bucket_offsets, bucket_curvature, n_buckets, h->stream,
-                                  h->err);
+    const uint32_t offs[2] = {0, n_in};
+    uint32_t scan_off[2], scan_bptr[2];
+    const int rc = preprocess_scans_device(1, pts_in, offs, leaf_size, nullptr, pts_out, scan_off, scan_bptr, bucket_offsets,
+                                           bucket_curvature, nullptr, h->pre_scratch, h->stream, h->err);
+    if (rc) return rc;
+    *n_out = scan_off[1];
+    *n_buckets = scan_bptr[1];
+    return LK_OK;
+}
+
+int lk_preprocess_scans(lk_handle h, uint32_t n_scans, const float* pts_in, const uint32_t* in_offsets, float leaf_size,
+                        const double* begin_times, float* pts_out, uint32_t* scan_offsets, uint32_t* scan_bucket_ptr,
+                        uint32_t* bucket_offsets, float* bucket_curvature, double* bucket_times) {
+    if (!h || !pts_in || !in_offsets || !pts_out || !scan_offsets || !scan_bucket_ptr || !bucket_offsets || !bucket_curvature)
+        return fail(h, LK_ERR_INVALID_ARG, "null argument");
+    if (!begin_times != !bucket_times) return fail(h, LK_ERR_INVALID_ARG, "begin_times and bucket_times go together");
+    if (!(leaf_size > 0) || !std::isfinite(leaf_size)) return fail(h, LK_ERR_INVALID_ARG, "leaf size must be positive and finite");
+    for (uint32_t s = 0; s < n_scans; ++s)
+        if (in_offsets[s + 1] < in_offsets[s]) return fail(h, LK_ERR_INVALID_ARG, "in_offsets not monotone");
+    if (!n_scans) {
+        scan_offsets[0] = scan_bucket_ptr[0] = bucket_offsets[0] = 0;
+        return LK_OK;
+    }
+    enter(h);
+    return preprocess_scans_device(n_scans, pts_in, in_offsets, leaf_size, begin_times, pts_out, scan_offsets, scan_bucket_ptr,
+                                   bucket_offsets, bucket_curvature, bucket_times, h->pre_scratch, h->stream, h->err);
 }
 
 int lk_leg_kinematics(lk_handle h, const lk_leg_cfg* cfg, const lk_leg_state* in, uint32_t n, int32_t redundancy,

@@ -73,6 +73,7 @@ def lib():
                                       vp, vp]
         L.lk_decode_pointcloud2.argtypes = [vp, vp, u32, vp, C.c_float, i32, dbl, vp, vp, vp, vp, vp]
         L.lk_preprocess_scan.argtypes = [vp, vp, u32, C.c_float, vp, vp, vp, vp, vp]
+        L.lk_preprocess_scans.argtypes = [vp, u32, vp, vp, C.c_float] + [vp] * 7
         L.lk_leg_track_default.argtypes = [vp]
         L.lk_leg_kinematics.argtypes = [vp, vp, vp, u32, i32, vp, vp, vp]
         _LIB = L
@@ -356,6 +357,32 @@ class Engine:
         no = np.zeros(1, np.uint32); nb = np.zeros(1, np.uint32)
         self._chk(lib().lk_preprocess_scan(self.h, _p(pts), n, leaf, _p(out), _p(no), _p(offs), _p(curv), _p(nb)))
         return out[:no[0]].copy(), offs[:nb[0] + 1].copy(), curv[:nb[0]].copy()
+
+    def preprocess_scans(self, pts, in_offsets, leaf, begin_times=None):
+        """lk_preprocess_scans: preprocess_scan of every scan of a batch in one call. pts float32 [n, 4] (x, y, z,
+        curvature), scan s = pts[in_offsets[s]:in_offsets[s + 1]]. Returns the batch layout scan_update / stage take:
+        pts, scan_offsets, scan_bucket_ptr, bucket_offsets, bucket_times (begin_times[s] + curvature; None when
+        begin_times is None) and bucket_curvature."""
+        pts = np.ascontiguousarray(pts, np.float32).reshape(-1, 4)
+        io = np.ascontiguousarray(in_offsets, np.uint32).reshape(-1)
+        if len(io) < 1:
+            raise ValueError("in_offsets needs n_scans + 1 entries")
+        if len(pts) < int(io[-1]):
+            raise ValueError(f"in_offsets ends at point {int(io[-1])}, pts has {len(pts)}")
+        n_scans = len(io) - 1
+        cap = max(int(io[-1]), 1)
+        out = np.zeros((cap, 4), np.float32); so = np.zeros(n_scans + 1, np.uint32); sbp = np.zeros(n_scans + 1, np.uint32)
+        bo = np.zeros(cap + 1, np.uint32); bc = np.zeros(cap, np.float32)
+        bt = None
+        if begin_times is not None:
+            begin_times = np.ascontiguousarray(begin_times, np.float64)
+            assert len(begin_times) == n_scans
+            bt = np.zeros(cap)
+        self._chk(lib().lk_preprocess_scans(self.h, n_scans, _p(pts), _p(io), leaf, _p(begin_times), _p(out), _p(so), _p(sbp),
+                                            _p(bo), _p(bc), _p(bt)))
+        n_out, n_b = int(so[-1]), int(sbp[-1])
+        return dict(pts=out[:n_out].copy(), scan_offsets=so, scan_bucket_ptr=sbp, bucket_offsets=bo[:n_b + 1].copy(),
+                    bucket_times=None if bt is None else bt[:n_b].copy(), bucket_curvature=bc[:n_b].copy())
 
     def leg_kinematics(self, states, cfg, track=None, redundancy=True):
         """lk_leg_kinematics: unitree HighState fields (abi.LEG_STATE_DTYPE) -> kinematic-inertial samples
