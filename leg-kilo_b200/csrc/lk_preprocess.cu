@@ -1,7 +1,8 @@
 // lk_preprocess.cu — what feeds the hot path (SURVEY §8f ranks 2-3), on the device:
 //   * wire decode of sensor_msgs/PointCloud2 for the three driver layouts
 //     (legkilo/src/preprocess/lidar_processing.cc:25-108): every filter_num-th point, blind-sphere test,
-//     time offset rounded to 1/500 s, stable compaction;
+//     time offset rounded to 1/500 s, stable compaction, begin / end times; a batch of messages in one pass
+//     (lk_decode_pointcloud2s; lk_decode_pointcloud2 is the batch of one);
 //   * pcl::VoxelGrid centroid down-sampling as KILO::process uses it (KILO.cc:82-83, :356-360; PCL 1.8
 //     voxel_grid.hpp — the library is absent from /root/reference, its published algorithm is restated),
 //     then the sort by curvature and the equal-curvature bucket boundaries (KILO.cc:370-378), for a batch of scans
@@ -12,6 +13,7 @@
 
 #include <algorithm>
 #include <climits>
+#include <cmath>
 #include <cstring>
 #include <string>
 #include <vector>
@@ -23,9 +25,22 @@ namespace lk {
 
 namespace {
 
-// ---- decode ---------------------------------------------------------------------------------------
-__global__ void k_decode_flags(const uint8_t* __restrict__ data, uint32_t n, lk_pc2_layout L, float blind,
-                               int filter_num, uint32_t* flags) {
+// ---- decode of a batch of messages ------------------------------------------------------------------
+// Message m is points [offs[m], offs[m+1]) of one device buffer (messages lie back to back, one layout), so point i is at
+// byte i * point_step. Every rule that depends on the message reads it through msg_of: the filter_num stride counts from
+// the message's own first point, and the time offset is taken from the message's own first raw point.
+__device__ __forceinline__ uint32_t msg_of(const uint32_t* __restrict__ offs, uint32_t n_msgs, uint32_t i) {
+    uint32_t lo = 0, hi = n_msgs;  // the last m with offs[m] <= i (an empty message m has offs[m] == offs[m + 1])
+    while (hi - lo > 1) {
+        const uint32_t mid = lo + (hi - lo) / 2;
+        if (offs[mid] <= i) lo = mid;
+        else hi = mid;
+    }
+    return lo;
+}
+
+__global__ void k_decode_flags(const uint8_t* __restrict__ data, const uint32_t* __restrict__ offs, uint32_t n_msgs, uint32_t n,
+                               lk_pc2_layout L, float blind, int filter_num, uint32_t* flags) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const uint8_t* p = data + (size_t)i * L.point_step;
@@ -33,7 +48,8 @@ __global__ void k_decode_flags(const uint8_t* __restrict__ data, uint32_t n, lk_
     memcpy(&x, p + L.off_x, 4); memcpy(&y, p + L.off_y, 4); memcpy(&z, p + L.off_z, 4);
     // blindCheck (lidar_processing.h:94-97): blind*blind > x*x + y*y + z*z, float, no contraction
     const float r2 = __fadd_rn(__fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y)), __fmul_rn(z, z));
-    const bool drop = (i % (uint32_t)filter_num) != 0 || (__fmul_rn(blind, blind) > r2);
+    const uint32_t k = i - offs[msg_of(offs, n_msgs, i)];
+    const bool drop = (k % (uint32_t)filter_num) != 0 || (__fmul_rn(blind, blind) > r2);
     flags[i] = drop ? 0u : 1u;
 }
 
@@ -43,15 +59,15 @@ __device__ __forceinline__ double raw_time(const uint8_t* p, const lk_pc2_layout
     double t; memcpy(&t, p + L.off_time, 8); return t;
 }
 
-__global__ void k_decode_scatter(const uint8_t* __restrict__ data, uint32_t n, lk_pc2_layout L, double time_scale,
-                                 const uint32_t* __restrict__ flags, const uint32_t* __restrict__ pos, float4* out,
-                                 float* intensity) {
+__global__ void k_decode_scatter(const uint8_t* __restrict__ data, const uint32_t* __restrict__ offs, uint32_t n_msgs, uint32_t n,
+                                 lk_pc2_layout L, double time_scale, const uint32_t* __restrict__ flags,
+                                 const uint32_t* __restrict__ pos, float4* out, float* intensity) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n || !flags[i]) return;
     const uint8_t* p = data + (size_t)i * L.point_step;
     float4 o;
     memcpy(&o.x, p + L.off_x, 4); memcpy(&o.y, p + L.off_y, 4); memcpy(&o.z, p + L.off_z, 4);
-    const double t0 = raw_time(data, L), ti = raw_time(p, L);
+    const double t0 = raw_time(data + (size_t)offs[msg_of(offs, n_msgs, i)] * L.point_step, L), ti = raw_time(p, L);
     if (L.lidar_type == LK_LIDAR_HESAI) {
         // double first / cur; std::round((cur - first) * 500.0f) / 500.0f in double, narrowed on store (:101-104)
         const double first = time_scale * t0, cur = time_scale * ti;
@@ -66,6 +82,33 @@ __global__ void k_decode_scatter(const uint8_t* __restrict__ data, uint32_t n, l
         float v; memcpy(&v, p + L.off_intensity, 4);
         intensity[pos[i]] = v;
     }
+}
+
+// Per message m <= n_msgs: its first output point (the exclusive sum at its first raw point; the total past the last
+// point), and for m < n_msgs lidar_begin_time_ / lidar_end_time_ (:31-35, :59-63, :87-91), NaN for an empty message.
+__global__ void k_decode_msgs(const uint8_t* __restrict__ data, const uint32_t* __restrict__ offs, uint32_t n_msgs, uint32_t n,
+                              lk_pc2_layout L, double time_scale, const double* __restrict__ stamps,
+                              const uint32_t* __restrict__ flags, const uint32_t* __restrict__ pos, uint32_t* out_offs,
+                              double* begin, double* end) {
+    const uint32_t m = blockIdx.x * blockDim.x + threadIdx.x;
+    if (m > n_msgs) return;
+    const uint32_t a = offs[m];
+    out_offs[m] = a < n ? pos[a] : pos[n - 1] + flags[n - 1];
+    if (m == n_msgs) return;
+    const uint32_t b = offs[m + 1];
+    double tb = __longlong_as_double(0x7ff8000000000000ll), te = tb;  // the quiet NaN std::nan("") gives on the host
+    if (b > a) {
+        const double f = time_scale * raw_time(data + (size_t)a * L.point_step, L);
+        const double l = time_scale * raw_time(data + (size_t)(b - 1) * L.point_step, L);
+        if (L.lidar_type == LK_LIDAR_HESAI) { tb = f; te = l; }  // no header stamp (:90-91)
+        else {
+            const double st = stamps ? stamps[m] : 0.0;  // stamp + float first / last point time (:34-35)
+            tb = st + (double)(float)f;
+            te = st + (double)(float)l;
+        }
+    }
+    begin[m] = tb;
+    end[m] = te;
 }
 
 // ---- voxel grid, time sort and buckets of a batch of scans -------------------------------------------------
@@ -242,41 +285,93 @@ struct PreScratch {
     }
 };
 
+
+// Device scratch of one lk_decode_pointcloud2s call, one block carved in this order: the raw bytes of n points, the
+// message offsets / stamps, keep flags and their exclusive sum, the decoded points, and the per-message outputs.
+struct DecScratch {
+    size_t data, offs, stamps, flags, pos, out, inten, out_offs, begin, end, tmp, total;
+    DecScratch(uint32_t n, uint32_t n_msgs, uint32_t point_step) {
+        size_t tb = 0;
+        cub::DeviceScan::ExclusiveSum(nullptr, tb, (const uint32_t*)nullptr, (uint32_t*)nullptr, (int)n);
+        size_t o = 0;
+        auto take = [&o](size_t bytes) { const size_t at = o; o += align_up(bytes); return at; };
+        data = take((size_t)n * point_step);
+        offs = take(((size_t)n_msgs + 1) * 4);
+        stamps = take((size_t)n_msgs * 8);
+        flags = take((size_t)n * 4);
+        pos = take((size_t)n * 4);
+        out = take((size_t)n * 16);
+        inten = take((size_t)n * 4);
+        out_offs = take(((size_t)n_msgs + 1) * 4);
+        begin = take((size_t)n_msgs * 8);
+        end = take((size_t)n_msgs * 8);
+        tmp = take(tb);
+        total = o;
+    }
+};
+
 }  // namespace
 
-int decode_pointcloud2_device(const uint8_t* h_data, uint32_t n, const lk_pc2_layout& L, float blind, int filter_num,
-                              double time_scale, float* h_pts_out, float* h_intensity_out, uint32_t* n_out, cudaStream_t s,
-                              std::string& err) {
-    *n_out = 0;
-    if (!n) return LK_OK;
-    DevBuf d_data, d_flags, d_pos, d_out, d_int, d_tmp;
-    const size_t bytes = (size_t)n * L.point_step;
-    LK_CUDA(err, d_data.alloc(bytes));
-    LK_CUDA(err, d_flags.alloc((size_t)n * 4));
-    LK_CUDA(err, d_pos.alloc((size_t)n * 4));
-    LK_CUDA(err, d_out.alloc((size_t)n * 16));
-    LK_CUDA(err, d_int.alloc((size_t)n * 4));
-    LK_CUDA(err, cudaMemcpyAsync(d_data.p, h_data, bytes, cudaMemcpyHostToDevice, s));
+// lk_decode_pointcloud2s behind its argument checks: n_msgs >= 1, every data[m] with points non-null, the sum of the
+// point counts at most INT_MAX. `scratch` is grown to the call's size. Two host synchronisations whatever n_msgs is: the
+// per-message offsets and times, then the copy-out of the points.
+int decode_pointcloud2s_device(uint32_t n_msgs, const uint8_t* const* h_data, const uint32_t* h_n, const double* h_stamps,
+                               const lk_pc2_layout& L, float blind, int filter_num, double time_scale, float* h_pts_out,
+                               float* h_intensity_out, uint32_t* h_out_offs, double* h_begin, double* h_end, DevBuf& scratch,
+                               cudaStream_t s, std::string& err) {
+    std::vector<uint32_t> offs(n_msgs + 1);
+    offs[0] = 0;
+    for (uint32_t m = 0; m < n_msgs; ++m) offs[m + 1] = offs[m] + h_n[m];
+    const uint32_t n = offs[n_msgs];
+    if (!n) {
+        const double nan = std::nan("");
+        for (uint32_t m = 0; m <= n_msgs; ++m) h_out_offs[m] = 0;
+        for (uint32_t m = 0; m < n_msgs; ++m) {
+            if (h_begin) h_begin[m] = nan;
+            if (h_end) h_end[m] = nan;
+        }
+        return LK_OK;
+    }
+    const DecScratch D(n, n_msgs, L.point_step);
+    LK_CUDA(err, scratch.ensure(D.total));
+    char* base_p = static_cast<char*>(scratch.p);
+    auto at = [base_p](size_t off) { return reinterpret_cast<void*>(base_p + off); };
+    auto* d_data = static_cast<uint8_t*>(at(D.data));
+    auto* d_offs = static_cast<uint32_t*>(at(D.offs));
+    auto* d_stamps = static_cast<double*>(at(D.stamps));
+    auto* d_flags = static_cast<uint32_t*>(at(D.flags));
+    auto* d_pos = static_cast<uint32_t*>(at(D.pos));
+    auto* d_out = static_cast<float4*>(at(D.out));
+    auto* d_int = static_cast<float*>(at(D.inten));
+    auto* d_out_offs = static_cast<uint32_t*>(at(D.out_offs));
+    auto* d_begin = static_cast<double*>(at(D.begin));
+    auto* d_end = static_cast<double*>(at(D.end));
+    size_t tb = D.total - D.tmp;
+
+    for (uint32_t m = 0; m < n_msgs; ++m)
+        if (h_n[m])
+            LK_CUDA(err, cudaMemcpyAsync(d_data + (size_t)offs[m] * L.point_step, h_data[m], (size_t)h_n[m] * L.point_step,
+                                         cudaMemcpyHostToDevice, s));
+    LK_CUDA(err, cudaMemcpyAsync(d_offs, offs.data(), offs.size() * 4, cudaMemcpyHostToDevice, s));
+    if (h_stamps) LK_CUDA(err, cudaMemcpyAsync(d_stamps, h_stamps, (size_t)n_msgs * 8, cudaMemcpyHostToDevice, s));
     const unsigned g = (n + 255) / 256;
-    k_decode_flags<<<g, 256, 0, s>>>(d_data.as<uint8_t>(), n, L, blind, filter_num, d_flags.as<uint32_t>());
-    size_t tb = 0;
-    cub::DeviceScan::ExclusiveSum(nullptr, tb, d_flags.as<uint32_t>(), d_pos.as<uint32_t>(), (int)n, s);
-    LK_CUDA(err, d_tmp.alloc(tb));
-    cub::DeviceScan::ExclusiveSum(d_tmp.p, tb, d_flags.as<uint32_t>(), d_pos.as<uint32_t>(), (int)n, s);
-    k_decode_scatter<<<g, 256, 0, s>>>(d_data.as<uint8_t>(), n, L, time_scale, d_flags.as<uint32_t>(), d_pos.as<uint32_t>(),
-                                       d_out.as<float4>(), h_intensity_out ? d_int.as<float>() : nullptr);
-    uint32_t last_pos = 0, last_flag = 0;
-    LK_CUDA(err, cudaMemcpyAsync(&last_pos, d_pos.as<uint32_t>() + (n - 1), 4, cudaMemcpyDeviceToHost, s));
-    LK_CUDA(err, cudaMemcpyAsync(&last_flag, d_flags.as<uint32_t>() + (n - 1), 4, cudaMemcpyDeviceToHost, s));
+    k_decode_flags<<<g, 256, 0, s>>>(d_data, d_offs, n_msgs, n, L, blind, filter_num, d_flags);
+    LK_CUDA(err, cub::DeviceScan::ExclusiveSum(at(D.tmp), tb, d_flags, d_pos, (int)n, s));
+    k_decode_scatter<<<g, 256, 0, s>>>(d_data, d_offs, n_msgs, n, L, time_scale, d_flags, d_pos, d_out,
+                                       h_intensity_out ? d_int : nullptr);
+    k_decode_msgs<<<(n_msgs + 256) / 256, 256, 0, s>>>(d_data, d_offs, n_msgs, n, L, time_scale, h_stamps ? d_stamps : nullptr,
+                                                      d_flags, d_pos, d_out_offs, d_begin, d_end);
+    LK_CUDA(err, cudaGetLastError());
+    LK_CUDA(err, cudaMemcpyAsync(h_out_offs, d_out_offs, ((size_t)n_msgs + 1) * 4, cudaMemcpyDeviceToHost, s));
+    if (h_begin) LK_CUDA(err, cudaMemcpyAsync(h_begin, d_begin, (size_t)n_msgs * 8, cudaMemcpyDeviceToHost, s));
+    if (h_end) LK_CUDA(err, cudaMemcpyAsync(h_end, d_end, (size_t)n_msgs * 8, cudaMemcpyDeviceToHost, s));
     LK_CUDA(err, cudaStreamSynchronize(s));
-    const uint32_t m = last_pos + last_flag;
-    *n_out = m;
-    if (m) {
-        LK_CUDA(err, cudaMemcpyAsync(h_pts_out, d_out.p, (size_t)m * 16, cudaMemcpyDeviceToHost, s));
-        if (h_intensity_out) LK_CUDA(err, cudaMemcpyAsync(h_intensity_out, d_int.p, (size_t)m * 4, cudaMemcpyDeviceToHost, s));
+    const uint32_t n_out = h_out_offs[n_msgs];
+    if (n_out) {
+        LK_CUDA(err, cudaMemcpyAsync(h_pts_out, d_out, (size_t)n_out * 16, cudaMemcpyDeviceToHost, s));
+        if (h_intensity_out) LK_CUDA(err, cudaMemcpyAsync(h_intensity_out, d_int, (size_t)n_out * 4, cudaMemcpyDeviceToHost, s));
         LK_CUDA(err, cudaStreamSynchronize(s));
     }
-    LK_CUDA(err, cudaGetLastError());
     return LK_OK;
 }
 

@@ -72,6 +72,7 @@ def lib():
         L.lk_process_scan.argtypes = [vp, vp, vp, vp, vp, vp, u32, vp, vp, u32, vp, vp, u32, dbl, dbl, i32, i32, vp,
                                       vp, vp]
         L.lk_decode_pointcloud2.argtypes = [vp, vp, u32, vp, C.c_float, i32, dbl, vp, vp, vp, vp, vp]
+        L.lk_decode_pointcloud2s.argtypes = [vp, u32, vp, vp, vp, vp, C.c_float, i32, dbl] + [vp] * 5
         L.lk_preprocess_scan.argtypes = [vp, vp, u32, C.c_float, vp, vp, vp, vp, vp]
         L.lk_preprocess_scans.argtypes = [vp, u32, vp, vp, C.c_float] + [vp] * 7
         L.lk_leg_track_default.argtypes = [vp]
@@ -348,6 +349,32 @@ class Engine:
         self._chk(lib().lk_decode_pointcloud2(self.h, _p(data), n, C.byref(layout), blind, filter_num, time_scale, _p(pts),
                                               _p(inten), _p(no), _p(ft), _p(lt)))
         return pts[:no[0]].copy(), inten[:no[0]].copy(), float(ft[0]), float(lt[0])
+
+    def decode_pointcloud2s(self, messages, layout, blind, filter_num, time_scale, stamps=None):
+        """lk_decode_pointcloud2s: decode_pointcloud2 of every message of a batch in one call. `messages` is a list of
+        uint8 arrays or structured point arrays (viewed as bytes here), each a whole number of layout.point_step points;
+        stamps [len(messages)] are the header stamps (None = 0). Returns pts float32 [n, 4], offsets [len(messages) + 1]
+        (message m is pts[offsets[m]:offsets[m + 1]]), intensity, begin_times and end_times, ready for
+        preprocess_scans(pts, offsets, leaf, begin_times)."""
+        step = layout.point_step
+        data = [np.ascontiguousarray(m).reshape(-1).view(np.uint8) for m in messages]
+        for i, d in enumerate(data):
+            if d.size % step:
+                raise ValueError(f"message {i} has {d.size} bytes, not a multiple of point_step {step}")
+        n_msgs = len(data)
+        if stamps is not None:
+            stamps = np.ascontiguousarray(stamps, np.float64).reshape(-1)
+            if len(stamps) != n_msgs:
+                raise ValueError(f"{len(stamps)} stamps for {n_msgs} messages")
+        ptrs = (C.c_void_p * max(n_msgs, 1))(*[d.ctypes.data for d in data])
+        counts = np.array([d.size // step for d in data], np.uint32)
+        cap = max(int(counts.sum(dtype=np.int64)), 1)
+        pts = np.zeros((cap, 4), np.float32); inten = np.zeros(cap, np.float32); offs = np.zeros(n_msgs + 1, np.uint32)
+        bt = np.zeros(n_msgs); et = np.zeros(n_msgs)
+        self._chk(lib().lk_decode_pointcloud2s(self.h, n_msgs, ptrs, _p(counts), _p(stamps), C.byref(layout), blind, filter_num,
+                                               time_scale, _p(pts), _p(inten), _p(offs), _p(bt), _p(et)))
+        n_out = int(offs[-1])
+        return dict(pts=pts[:n_out].copy(), offsets=offs, intensity=inten[:n_out].copy(), begin_times=bt, end_times=et)
 
     def preprocess_scan(self, pts, leaf):
         """lk_preprocess_scan: voxel-grid centroid filter, stable curvature sort, bucket boundaries."""

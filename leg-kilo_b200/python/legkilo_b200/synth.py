@@ -211,6 +211,50 @@ VLP16 = dict(n_rings=16, n_az=1800, fov_deg=(-15.0, 15.0))
 OS64 = dict(n_rings=64, n_az=2048, fov_deg=(-16.6, 16.6))
 
 
+# Raw time units of the three drivers' shipped configurations (nclt / diter / hilti .yaml): the time_scale of each.
+PC2_TIME_SCALE = {1: 1e-6, 2: 1e-9, 3: 1.0}
+
+
+def pack_pointcloud2(lidar_type: int, xyz, t, intensity, t0: float = 0.0) -> np.ndarray:
+    """One PointCloud2 message's points in the driver layout abi.PC2_DTYPES[lidar_type] (its .view(np.uint8) is the
+    message's data). xyz [n, 3], t [n] seconds since the start of the sweep, raw time as the driver writes it
+    (lidar_processing.h:10-72): Velodyne float32 microseconds, Ouster uint32 nanoseconds, Hesai float64 absolute
+    seconds t0 + t."""
+    from . import abi
+    xyz = np.asarray(xyz, np.float32).reshape(-1, 3)
+    a = np.zeros(len(xyz), abi.PC2_DTYPES[lidar_type])
+    a["x"], a["y"], a["z"] = xyz[:, 0], xyz[:, 1], xyz[:, 2]
+    a["intensity"] = intensity
+    t = np.asarray(t, np.float64)
+    if lidar_type == 1:
+        a["time"] = (t * 1e6).astype(np.float32)
+    elif lidar_type == 2:
+        a["t"] = np.round(t * 1e9).astype(np.uint32)
+    else:
+        a["timestamp"] = t0 + t
+    return a
+
+
+def box_pointcloud2s(n_msgs: int, lidar_type: int, lidar=VLP16, distinct: int = 8, stream: int = 9500):
+    """n_msgs PointCloud2 messages of box-room sweeps (`distinct` poses, repeated) in the driver layout of `lidar_type`,
+    with the ray geometry of `lidar`. Raw point times jitter by up to 1 ms around each ray's firing time, so the decode's
+    2 ms rounding has work to do; no blind cut, so points near the sensor stay in. Returns (messages as structured arrays,
+    header stamps 1000 + 0.1 s per message)."""
+    from . import abi
+    R, t = abi.extrinsics(abi.CONFIGS["leg_fusion"])
+    sc = BoxScene(ground_half_extent=20.0)
+    rv, tv = random_poses(distinct, 0.2, 2.0, stream=stream)
+    stamps = 1000.0 + 0.1 * np.arange(n_msgs)
+    base = []
+    for i in range(distinct):
+        g = rng(stream + 1 + distinct + i)
+        s = sc.scan(rotvec=rv[i], trans=tv[i], ext_R=R, ext_t=t, blind=0.0, stream=stream + 1 + i, streaming=True, **lidar)
+        tt = np.clip(s[:, 3].astype(np.float64) + g.uniform(-1e-3, 1e-3, len(s)), 0.0, None)
+        base.append((s[:, :3], tt, g.uniform(0.0, 255.0, len(s)).astype(np.float32)))
+    msgs = [pack_pointcloud2(lidar_type, *base[m % distinct], t0=stamps[m]) for m in range(n_msgs)]
+    return msgs, stamps
+
+
 def random_poses(batch: int, rot_sigma: float, trans_sigma: float, stream: int = 31):
     g = rng(stream)
     return rot_sigma * g.standard_normal((batch, 3)), trans_sigma * g.standard_normal((batch, 3))
