@@ -17,9 +17,11 @@ G_ROTVEC = (0.35, -0.6, 1.1)
 G_POS = (-37.3, 81.6, 2.4)
 FAR_POS = (1800.3, -2600.7, 35.2)
 
-# State / covariance tolerance of a whole streaming frame with map updates at a dense prior: the reference itself moves
-# by up to a few 1e-7 of the update step when P0 changes by 1e-15 (tests/golden/make_ref_general_golden.py checks it)
-STREAM_TOL = 5e-6
+# (state_err, cov_err) tolerances (tests/scenes.py) of a whole streaming frame with map updates at a dense prior. Such a
+# frame is sensitive: when P0 changes by 1e-15 the reference itself moves by up to 3.1e-5 sd / 5.2e-8
+# (tests/golden/make_ref_general_golden.py checks that these moves stay within a quarter of the tolerances). Measured worst:
+# the oracle against the fixtures 2.1e-5 sd / 3.9e-8, the device on an H100 80GB HBM3 3.2e-5 sd / 6.8e-8.
+STREAM_TOLS = (1e-3, 2e-6)
 
 # state blocks of the 30-vector (eskf.h): rot, pos, vel, ba, bw, grav, imu_a, imu_w, bv, contact
 _SD_REST = (0.02, 0.02, 0.02, 5e-3, 5e-3, 5e-3, 1e-3, 1.2e-3, 0.8e-3, 1e-3, 1e-3, 1e-3, 0.05, 0.05, 0.05, 0.01, 0.01, 0.01,
@@ -103,16 +105,6 @@ def map_covs(G):
     """Non-isotropic attitude / position covariances for BuildVoxelMap (the first frame's P blocks)."""
     A = synth.exp_so3((0.3, 0.2, -0.4))
     return A @ np.diag([1e-6, 2.5e-6, 4e-6]) @ A.T, G @ np.diag([3e-6, 1e-6, 6e-6]) @ G.T
-
-
-def rel_state(xa, xb, x0):
-    import lko
-    return np.abs(lko.boxminus(xa, xb)).max() / max(np.abs(lko.boxminus(xb, x0)).max(), 1e-12)
-
-
-def rel_cov(Pa, Pb):
-    Pa, Pb = np.asarray(Pa).ravel(), np.asarray(Pb).ravel()
-    return np.abs(Pa - Pb).max() / np.abs(Pb).max()
 
 
 def world_atol(world, floor=5e-6):

@@ -23,9 +23,13 @@ for p in ("leg-kilo_b200/python", "oracle", "tests"):
 import general_prior as gp  # noqa: E402
 import lkref  # noqa: E402
 import mapcmp  # noqa: E402
+import scenes  # noqa: E402
 from legkilo_b200 import abi, synth  # noqa: E402
 
 G = synth.exp_so3(gp.G_ROTVEC)
+# (state_err, cov_err) by which the reference's output for the skewed P0 must differ from its output for the symmetric part
+# (measured: 2.7e-4 sd, 1.2e-3)
+SKEW_SEEN = (1e-5, 1e-4)
 
 
 def _reference(cfg, pw, pb, imu_mode_only=True):
@@ -61,8 +65,8 @@ def bucket(cfg_name, pos=gp.G_POS, asym=False):
         Psym = 0.5 * (P0.reshape(30, 30) + P0.reshape(30, 30).T)
         rs, _, _ = run(Psym.ravel())
         xs, Ps, _, _ = rs.get_filter()
-        # (the covariance is measured against its largest entry, which the predict's Q dt^2 on imu_a makes ~50x P0's)
-        assert gp.rel_state(xs, x, x0) > 1e-6 and gp.rel_cov(Ps, P) > 1e-9, (gp.rel_state(xs, x, x0), gp.rel_cov(Ps, P))
+        es, eP = scenes.state_err(xs, x, P), scenes.cov_err(Ps, P)
+        assert es > SKEW_SEEN[0] and eP > SKEW_SEEN[1], (es, eP)
     name = "asym" if asym else ("far" if pos is gp.FAR_POS else cfg_name)
     np.savez_compressed(os.path.join(HERE, f"ref_general_bucket_{name}.npz"), pw=pw, pb=pb, map0=map0, x0=x0.view(np.float64),
                         P0=P0, clk0=clk.view(np.float64), t=100.0, pts=pts, x=x.view(np.float64), P=P, clk=c.view(np.float64),
@@ -91,13 +95,13 @@ def stream(kind):
     x, P, _, c = r.get_filter()
     # At a dense prior, the map update makes a frame of ~50 buckets sensitive: a change of 1e-15 in P0 moves the final
     # state of the reference itself by up to a few 1e-7 of the update step (without UpdateVoxelMap, by 1e-16). The
-    # tests compare these fixtures to STREAM_TOL; the generator checks that three such perturbations stay well inside it.
+    # tests compare these fixtures to STREAM_TOLS; the generator checks that three such perturbations stay well inside it.
     for s in (9297, 9298, 9299):
         Pp = P0 * (1.0 + 1e-15 * synth.rng(s).standard_normal(900))
         rp, _, _ = run((0.5 * (Pp.reshape(30, 30) + Pp.reshape(30, 30).T)).ravel())
         xp, Ppp, _, _ = rp.get_filter()
-        spread = max(gp.rel_state(xp, x, x0), gp.rel_cov(Ppp, P))
-        assert spread < gp.STREAM_TOL / 4, spread
+        spread = scenes.state_err(xp, x, P), scenes.cov_err(Ppp, P)
+        assert spread[0] < gp.STREAM_TOLS[0] / 4 and spread[1] < gp.STREAM_TOLS[1] / 4, spread
     np.savez_compressed(os.path.join(HERE, f"ref_general_stream_{kind}.npz"), pw=pw, pb=pb, map0=map0, x0=x0.view(np.float64), P0=P0,
                         clk0=clk.view(np.float64), begin=20.0, pts=out["body"], meas=meas.view(np.uint8), x=x.view(np.float64), P=P,
                         clk=c.view(np.float64), world=out["world"], n_eff=out["n_eff"], map1=mapcmp.digest(r.map_export()))

@@ -8,7 +8,8 @@ import scenes
 from legkilo_b200 import Engine, LkError, abi
 
 pytestmark = pytest.mark.gpu
-TOL = 1e-5
+STATE_TOL = 7e-12  # (tests/scenes.py) worst measured on an H100 80GB HBM3: 7.2e-14 sd
+COV_TOL = 1.9e-12  # worst measured: 1.9e-14
 
 
 def _oracle(cfg, blob, pts, x0, P0, iters):
@@ -48,8 +49,7 @@ def test_ragged_batch_with_empty_and_far_away_scans():
     for i in (0, 2):
         ro, xo, Po = _oracle(cfg, blob, pieces[i], x0[i:i + 1], P0[i:i + 1], 2)
         assert int(out["n_eff"][i]) == ro["n_eff"] > 0
-        assert scenes.rel_state_err(out["x"][i:i + 1], xo, x0[i:i + 1]) < TOL
-        assert scenes.rel_cov_err(out["P"][i], Po) < TOL
+        scenes.check_filter(out["x"][i:i + 1], out["P"][i], xo, Po, STATE_TOL, COV_TOL, f"scan {i}")
     for i in (1, 3):
         assert int(out["n_eff"][i]) == 0
         np.testing.assert_array_equal(out["x"][i:i + 1].view(np.float64), x0[i:i + 1].view(np.float64))
@@ -85,7 +85,7 @@ def test_argument_errors_are_status_codes_and_the_handle_survives():
     out = eng.scan_update(x1, P1, Q, c1, s, [0, len(s)], [0.0], iters=2)
     ro, xo, Po = _oracle(cfg, blob, s, x1, P1, 2)
     assert int(out["n_eff"][0]) == ro["n_eff"] > 0
-    assert scenes.rel_state_err(out["x"], xo, x1) < TOL
+    scenes.check_filter(out["x"], out["P"][0], xo, Po, STATE_TOL, COV_TOL)
 
 
 def test_corrupt_map_blobs_are_rejected():

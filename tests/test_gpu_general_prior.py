@@ -11,12 +11,20 @@ import pytest
 import general_prior as gp
 import lko
 import mapcmp
+import scenes
 from legkilo_b200 import Engine, abi, shard, synth
 
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 G = synth.exp_so3(gp.G_ROTVEC)
-TOL = 1e-8  # device (information form) against the oracle in the same form, static map
+# (state_err, cov_err) tolerances (tests/scenes.py), each 100x the worst measured on an H100 80GB HBM3:
+# - the device (information form) against the oracle in the same form, static map: 6.7e-12 sd, 2.9e-14;
+# - heterogeneous batches, whose streaming scans carry absolute stamps of 1.7e9 s: 1.6e-9 sd, 2.5e-11;
+# - the reference-made bucket fixtures (literal gain, with UpdateVoxelMap): 4.2e-8 sd, 9.9e-12.
+STATE_TOL = 6e-10
+COV_TOL = 2.9e-12
+HETERO_TOLS = (1.5e-7, 2.5e-9)
+FIXTURE_TOLS = (4e-6, 9e-10)
 
 
 def _load(name):
@@ -28,10 +36,9 @@ def _load(name):
     return d
 
 
-def _check_fixture(d, x, P, clk, world, n_eff, blob, tol, center_atol, map_rtol=1e-5, d_atol=1e-5, radius_rtol=1e-6):
+def _check_fixture(d, x, P, clk, world, n_eff, blob, tols, center_atol, map_rtol=1e-5, d_atol=1e-5, radius_rtol=1e-6):
     assert int(n_eff) == int(d["n_eff"]) > 0
-    assert gp.rel_state(x, d["x"], d["x0"]) < tol, gp.rel_state(x, d["x"], d["x0"])
-    assert gp.rel_cov(P, d["P"]) < tol, gp.rel_cov(P, d["P"])
+    scenes.check_filter(x, P, d["x"], d["P"], *tols)
     assert np.asarray(clk).tobytes() == d["clk"].tobytes()
     err = np.abs(world[:, :3] - d["world"][:, :3])
     assert (err <= gp.world_atol(d["world"])).all(), err.max()
@@ -105,7 +112,7 @@ def test_bucket_fixture_on_device_paths(name, path, params, pinned):
     n = len(d["pts"])
     out = eng.scan_update(d["x0"], d["P0"], abi.process_cov_Q(cfg), d["clk0"], d["pts"], [0, n], [float(d["t"])], iters=1,
                           update_map=True, pinned=pinned)
-    _check_fixture(d, out["x"], out["P"][0], out["clk"], np.asarray(out["world"]), out["n_eff"][0], eng.map_download(), 1e-7,
+    _check_fixture(d, out["x"], out["P"][0], out["clk"], np.asarray(out["world"]), out["n_eff"][0], eng.map_download(), FIXTURE_TOLS,
                    1e-8 * scale, map_rtol=1e-5 * far, radius_rtol=1e-6 * far)
 
 
@@ -120,7 +127,7 @@ def test_stream_fixture_process_scan(kind, insert):
     assert pts.tobytes() == d["pts"].tobytes()
     out = eng.process_scan(d["x0"], d["P0"], abi.process_cov_Q(cfg), d["clk0"], pts, offs, times, imu=meas if kind == "imu" else None,
                            kin=meas if kind == "kin" else None, gravity=9.81, acc_norm=9.79, iters=1, update_map=True)
-    _check_fixture(d, out["x"], out["P"], out["clk"], out["world"], out["n_eff"], eng.map_download(), gp.STREAM_TOL, 1e-6,
+    _check_fixture(d, out["x"], out["P"], out["clk"], out["world"], out["n_eff"], eng.map_download(), gp.STREAM_TOLS, 1e-6,
                    map_rtol=1e-4, d_atol=1e-3)
 
 
@@ -204,8 +211,7 @@ def test_scan_update_against_oracle(iters, streaming, asym):
         eng.map_upload(blob)
         out = eng.scan_update(x0, P0, abi.process_cov_Q(cfg), clk0, pts, [0, len(pts)], times, iters=iters, **kw)
         assert int(out["n_eff"][0]) == ro["n_eff"] > 0
-        assert gp.rel_state(out["x"], xo, x0) < TOL, gp.rel_state(out["x"], xo, x0)
-        assert gp.rel_cov(out["P"][0], Po) < TOL, gp.rel_cov(out["P"][0], Po)
+        scenes.check_filter(out["x"], out["P"][0], xo, Po, STATE_TOL, COV_TOL, f"fused {fused}")
         np.testing.assert_array_equal(out["clk"].view(np.float64), clko.view(np.float64))
         err = np.abs(out["world"][:, :3] - ro["world"][:, :3])
         assert (err <= gp.world_atol(ro["world"])).all(), err.max()
@@ -292,8 +298,7 @@ def test_heterogeneous_batch(streaming):
         assert out["clk"][i].tobytes() == clko.tobytes(), i
         if ro["n_eff"] > 0:
             some += 1
-            assert gp.rel_state(out["x"][i:i + 1], xo, x0[i:i + 1]) < 1e-7, (i, gp.rel_state(out["x"][i:i + 1], xo, x0[i:i + 1]))
-            assert gp.rel_cov(out["P"][i], Po) < 1e-7, (i, gp.rel_cov(out["P"][i], Po))
+            scenes.check_filter(out["x"][i:i + 1], out["P"][i], xo, Po, *HETERO_TOLS, f"scan {i} of {len(p)} points")
         err = np.abs(out["world"][so[i]:so[i + 1], :3] - ro["world"][:, :3])
         assert (err <= gp.world_atol(ro["world"])).all(), (i, err.max())
     assert some >= B - 2
@@ -350,7 +355,7 @@ def test_far_from_origin_paths():
         eng.set_param("fused", fused)
         out = eng.scan_update(x0, P0, Q, clk0, pts, [0, len(pts)], [100.0], iters=2)
         assert int(out["n_eff"][0]) == rb["n_eff"]
-        assert gp.rel_state(out["x"], xo, x0) < TOL and gp.rel_cov(out["P"][0], Po) < TOL
+        scenes.check_filter(out["x"], out["P"][0], xo, Po, STATE_TOL, COV_TOL, f"fused {fused}")
         err = np.abs(out["world"][:, :3] - rb["world"][:, :3])
         assert (err <= gp.world_atol(rb["world"])).all(), err.max()
     # the batched path: the far scan next to a copy of it at another prior
@@ -361,4 +366,4 @@ def test_far_from_origin_paths():
     for i in range(2):
         rb, xo, Po, _ = _oracle_bucket(cfg, blob, pts, x2[i:i + 1], P2[i], clk0, 100.0, iters=2)
         assert int(out["n_eff"][i]) == rb["n_eff"] > 0
-        assert gp.rel_state(out["x"][i:i + 1], xo, x2[i:i + 1]) < TOL and gp.rel_cov(out["P"][i], Po) < TOL
+        scenes.check_filter(out["x"][i:i + 1], out["P"][i], xo, Po, STATE_TOL, COV_TOL, f"batched scan {i}")

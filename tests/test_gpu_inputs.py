@@ -12,7 +12,8 @@ import scenes
 from legkilo_b200 import Engine, abi, synth
 
 pytestmark = pytest.mark.gpu
-TOL = 1e-5
+STATE_TOL = 6e-12  # (tests/scenes.py) worst measured on an H100 80GB HBM3: 6.5e-14 sd
+COV_TOL = 1.2e-12  # worst measured: 1.2e-14
 
 
 def _oracle(cfg, blob, pts, x0, P0, iters):
@@ -54,8 +55,7 @@ def _check_all_paths(cfg, blob, pts, x0=None, iters=3, min_frac=0.5, expect_rows
     for name, out, i in (("fused", outs[1], 0), ("multi-kernel", outs[0], 0), ("batched[0]", two, 0), ("batched[1]", two, 1)):
         assert int(out["n_eff"][i]) == ro["n_eff"], name
         if ro["n_eff"] > 0:
-            assert scenes.rel_state_err(out["x"][i:i + 1], xo, x0) < TOL, name
-            assert scenes.rel_cov_err(out["P"][i], Po) < TOL, name
+            scenes.check_filter(out["x"][i:i + 1], out["P"][i], xo, Po, STATE_TOL, COV_TOL, name)
         else:
             assert out["x"][i:i + 1].tobytes() == x0.tobytes(), name
             np.testing.assert_array_equal(out["P"][i], P0[0], err_msg=name)

@@ -8,6 +8,9 @@ import scenes
 from legkilo_b200 import Engine, abi, synth
 
 pytestmark = pytest.mark.gpu
+# streaming scans with UpdateVoxelMap, device against the oracle
+STATE_TOL = 7e-6  # (tests/scenes.py) worst measured on an H100 80GB HBM3: 7.0e-8 sd (the map built from an empty one)
+COV_TOL = 4.5e-7  # worst measured: 4.6e-9
 
 
 def _both(cfg, pw, pb, R=None, rot_cov=None, pos_cov=None):
@@ -89,8 +92,7 @@ def _stream_case(streaming, iters=1, stream0=700, empty_map=False, n_scans=2, fa
                               bucket_offsets=offs, iters=iters, update_map=True)
         xo, Po, _, clko = o.get_filter()
         assert int(out["n_eff"][0]) == ro["n_eff"]
-        assert scenes.rel_state_err(out["x"], xo, x0) < 1e-5
-        assert scenes.rel_cov_err(out["P"][0], Po) < 1e-5
+        scenes.check_filter(out["x"], out["P"][0], xo, Po, STATE_TOL, COV_TOL, f"scan at {t0:.1f}")
         if check_world:  # the re-projected cloud comes out of the insert's first phase on the fast path
             np.testing.assert_allclose(out["world"][:, :3], ro["world"][:, :3], rtol=0, atol=5e-6)
             np.testing.assert_array_equal(out["world"][:, 3], ro["world"][:, 3])

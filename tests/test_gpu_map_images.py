@@ -24,7 +24,8 @@ import test_gpu_parity as tp
 from legkilo_b200 import Engine, abi, synth
 
 pytestmark = pytest.mark.gpu
-TOL = 1e-5
+STATE_TOL = 2.4e-11  # (tests/scenes.py) worst measured on an H100 80GB HBM3 (here and in test_gpu_map_insert.py): 2.4e-13 sd
+COV_TOL = 1.3e-10  # worst measured: 1.3e-12
 ITERS = 2
 PROBE_LIDAR = dict(n_rings=16, n_az=900, fov_deg=(-15.0, 15.0))  # ~14 000 points: one 256-point chunk per block
 # the insert paths of update_map calls: (fast_insert, fused_insert)
@@ -222,8 +223,7 @@ def _probe(eng, cfg, pts, x0, P0=None):
             assert int(out["n_eff"][i]) == ro2["n_eff"], (k, i, out["n_eff"], ro2["n_eff"])
             if ro2["n_eff"] == 0:
                 continue
-            assert scenes.rel_state_err(out["x"][i:i + 1], xo, x0) < TOL, k
-            assert scenes.rel_cov_err(out["P"][i], Po) < TOL, k
+            scenes.check_filter(out["x"][i:i + 1], out["P"][i], xo, Po, STATE_TOL, COV_TOL, f"fused {k} scan {i}")
     _same({k: st[1][k] for k in ("x", "P", "n_eff")}, st[0], "fused 1 vs 0")
     # d. a second handle whose images come from k_hot_from_nodes: every output bitwise
     twin = Engine(cfg)

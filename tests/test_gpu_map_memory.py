@@ -9,6 +9,9 @@ import scenes
 from legkilo_b200 import Engine, abi, synth
 
 pytestmark = pytest.mark.gpu
+# one streaming scan with UpdateVoxelMap from a common prior, device against the oracle
+STATE_TOL = 4.8e-4  # (tests/scenes.py) worst measured on an H100 80GB HBM3: 4.9e-6 sd, a scan into a map of frozen leaves
+COV_TOL = 3.9e-6  # worst measured: 4.0e-8
 
 LIDAR = dict(n_rings=8, n_az=450, fov_deg=(-15.0, 15.0))  # ~3 000 points per revolution, 50 buckets of 2 ms
 N_FROZEN = 200
@@ -58,8 +61,7 @@ class _Stream:
             ro = self.o.process_scan(self.t0, pts)
             xo, Po, _, _ = self.o.get_filter()
             assert int(out["n_eff"][0]) == ro["n_eff"]
-            assert scenes.rel_state_err(out["x"], xo, self.x0) < 1e-5
-            assert scenes.rel_cov_err(out["P"][0], Po) < 1e-5
+            scenes.check_filter(out["x"], out["P"][0], xo, Po, STATE_TOL, COV_TOL, f"scan at {self.t0:.1f}")
         self.x, self.P, self.clk = out["x"], out["P"], out["clk"]
         self.t0 += 0.1
         return out

@@ -1,6 +1,6 @@
 """GPU parity: the CUDA path through the C ABI against the CPU oracle on identical inputs.
-Tolerance: 1e-5 relative on the 30-vector state (via State [-]) and on the 30x30 covariance
-(BASELINE.json north_star); in practice the paths agree to ~1e-10."""
+States are compared in posterior standard deviations and covariances in correlation units (scenes.state_err /
+scenes.cov_err), so that the pose block is held to the same standard as the large imu_w / imu_a variances."""
 import numpy as np
 import pytest
 
@@ -9,7 +9,12 @@ import scenes
 from legkilo_b200 import Engine, abi, synth
 
 pytestmark = pytest.mark.gpu
-TOL = 1e-5
+# (state_err, cov_err) tolerances, 100x the worst measured on an H100 80GB HBM3: 5.6e-11 sd (the throughput family, a 2 047-point scan,
+# 2 iterations) and 1.7e-14 with a static map; 2.1e-9 sd and 4.0e-12 for the streaming fixture with UpdateVoxelMap
+STATE_TOL = 5e-9
+COV_TOL = 1e-12
+MAP_STATE_TOL = 2e-7
+MAP_COV_TOL = 4e-10
 
 
 def _oracle_bucket(cfg, blob, pts, x0, P0, iters=1, gain=lko.GAIN_INFORMATION, t=0.0):
@@ -32,8 +37,7 @@ def test_config1_planar_literal_pin():
     eng.map_upload(blob)
     out = eng.scan_update(x0, P0, abi.process_cov_Q(cfg), np.zeros(1, abi.CLOCK_DTYPE), pts, [0, len(pts)], [0.0])
     assert int(out["n_eff"][0]) == ro["n_eff"] > 0.9 * len(pts)
-    assert scenes.rel_state_err(out["x"], xo, x0) < TOL
-    assert scenes.rel_cov_err(out["P"][0], Po) < TOL
+    scenes.check_filter(out["x"], out["P"][0], xo, Po, STATE_TOL, COV_TOL)
     np.testing.assert_allclose(out["world"][:, :3], ro["world"][:, :3], rtol=0, atol=2e-6)
     assert np.all(out["world"][:, 3] == 255.0)
     assert out["clk"]["last_update_time"][0] == clko["last_update_time"][0]
@@ -75,8 +79,7 @@ def test_box_room_batch(iters):
     for i, s in enumerate(scans):
         ro, xo, Po, _ = _oracle_bucket(cfg, blob, s, x0[i:i + 1], P0[i:i + 1], iters=iters)
         assert int(out["n_eff"][i]) == ro["n_eff"] > 0
-        assert scenes.rel_state_err(out["x"][i:i + 1], xo, x0[i:i + 1]) < TOL
-        assert scenes.rel_cov_err(out["P"][i], Po) < TOL
+        scenes.check_filter(out["x"][i:i + 1], out["P"][i], xo, Po, STATE_TOL, COV_TOL, f"scan {i}")
 
 
 @pytest.mark.parametrize("fused", [0, 1])
@@ -91,8 +94,7 @@ def test_single_scan_paths_agree_with_oracle(fused):
     out = eng.scan_update(x0, P0, abi.process_cov_Q(cfg), np.zeros(1, abi.CLOCK_DTYPE), scans[0], [0, len(scans[0])], [0.0], iters=3)
     ro, xo, Po, _ = _oracle_bucket(cfg, blob, scans[0], x0, P0, iters=3)
     assert int(out["n_eff"][0]) == ro["n_eff"] > 0
-    assert scenes.rel_state_err(out["x"], xo, x0) < TOL
-    assert scenes.rel_cov_err(out["P"][0], Po) < TOL
+    scenes.check_filter(out["x"], out["P"][0], xo, Po, STATE_TOL, COV_TOL)
     np.testing.assert_allclose(out["world"][:, :3], ro["world"][:, :3], rtol=0, atol=2e-6)
     key = "_single_scan_ref"
     if key in globals():
@@ -132,8 +134,7 @@ def test_throughput_family_chunk_edges():
         assert int(out["n_eff"][i]) == ro["n_eff"], (ws, len(s))
         if ro["n_eff"] > 0:
             some += 1
-            assert scenes.rel_state_err(out["x"][i:i + 1], xo, x0[i:i + 1]) < TOL, (ws, len(s))
-            assert scenes.rel_cov_err(out["P"][i], Po) < TOL, (ws, len(s))
+            scenes.check_filter(out["x"][i:i + 1], out["P"][i], xo, Po, STATE_TOL, COV_TOL, f"{len(s)} points")
         np.testing.assert_allclose(out["world"][offs[i]:offs[i + 1], :3], ro["world"][:, :3], rtol=0, atol=5e-6)
     assert some >= len(sizes) - 3
     # many small scans: more chunks than SMs, so the persistent variant walks several chunks per block (stage ring
@@ -153,8 +154,7 @@ def test_throughput_family_chunk_edges():
         ro, xo, Po, _ = _oracle_bucket(cfg, blob, pieces2[i], x2[i:i + 1], P2[i:i + 1], iters=2)
         assert int(out2["n_eff"][i]) == ro["n_eff"], (ws, i)
         if ro["n_eff"] > 0:
-            assert scenes.rel_state_err(out2["x"][i:i + 1], xo, x2[i:i + 1]) < TOL, (ws, i)
-            assert scenes.rel_cov_err(out2["P"][i], Po) < TOL, (ws, i)
+            scenes.check_filter(out2["x"][i:i + 1], out2["P"][i], xo, Po, STATE_TOL, COV_TOL, f"scan {i} of {B2}")
 
 
 @pytest.mark.parametrize("streaming", [False, True])
@@ -242,8 +242,7 @@ def test_streaming_buckets_static_map(fused, iters):
     out = eng.scan_update(x0, P0, abi.process_cov_Q(cfg), clk0, pts, [0, len(pts)], times, scan_bucket_ptr=[0, len(times)],
                           bucket_offsets=offs, iters=iters)
     assert int(out["n_eff"][0]) == ro["n_eff"] > 0
-    assert scenes.rel_state_err(out["x"], xo, x0) < TOL
-    assert scenes.rel_cov_err(out["P"][0], Po) < TOL
+    scenes.check_filter(out["x"], out["P"][0], xo, Po, STATE_TOL, COV_TOL)
     assert out["clk"]["last_predict_time"][0] == clko["last_predict_time"][0]
     assert out["clk"]["last_update_time"][0] == clko["last_update_time"][0]
     np.testing.assert_allclose(out["world"][:, :3], ro["world"][:, :3], rtol=0, atol=5e-6)
@@ -263,7 +262,7 @@ def test_golden_fixtures_on_gpu():
     out = eng.scan_update(x0, P0, abi.process_cov_Q(cfg), np.zeros(1, abi.CLOCK_DTYPE), pts, [0, len(pts)], [0.0])
     xg = g["x"].view(abi.STATE_DTYPE)
     assert int(out["n_eff"][0]) == int(g["n_eff"])
-    assert scenes.rel_state_err(out["x"], xg, x0) < TOL and scenes.rel_cov_err(out["P"][0], g["P"]) < TOL
+    scenes.check_filter(out["x"], out["P"][0], xg, g["P"], STATE_TOL, COV_TOL, "config1_planar")
 
     g = np.load(os.path.join(gdir, "streaming_box.npz"))
     cfg, blob, scans = scenes.box_scene(batch=1, streaming=True, stream0=700, ground_half_extent=12.0)
@@ -274,8 +273,7 @@ def test_golden_fixtures_on_gpu():
     out = eng.scan_update(x0, P0, abi.process_cov_Q(cfg), clk, pts, [0, len(pts)], times, scan_bucket_ptr=[0, len(times)],
                           bucket_offsets=offs, update_map=True)
     assert int(out["n_eff"][0]) == int(g["n_eff"])
-    assert scenes.rel_state_err(out["x"], g["x"].view(abi.STATE_DTYPE), x0) < TOL
-    assert scenes.rel_cov_err(out["P"][0], g["P"]) < TOL
+    scenes.check_filter(out["x"], out["P"][0], g["x"].view(abi.STATE_DTYPE), g["P"], MAP_STATE_TOL, MAP_COV_TOL, "streaming_box")
     np.testing.assert_array_equal(out["clk"].view(np.float64), g["clk"])
     st = eng.map_stats()
     assert st["roots"] == int(g["n_roots"]) and st["nodes"] >= int(g["n_nodes"]) and st["points"] == int(g["n_points"])

@@ -139,6 +139,10 @@ def test_oracle_matches_reference_golden():
 # ---- GPU ----------------------------------------------------------------------------------------------------------
 
 FK_TOL = 1e-12
+# three streaming scans with map updates, the device filter carried from scan to scan, against the oracle's
+# (tests/scenes.py; worst measured on an H100 80GB HBM3: 5.2e-9 sd, 4.1e-12)
+KIN_CHAIN_STATE_TOL = 5e-7
+KIN_CHAIN_COV_TOL = 4e-10
 
 
 @pytest.fixture(scope="module")
@@ -275,5 +279,5 @@ def test_gpu_three_streaming_scans_kin_imu_mode():
         qg = qg[out["n_consumed"]:]; qo = qo[ro["n_consumed"]:]
         x, P, c = out["x"], out["P"], out["clk"]
         xo, Po, _, co = o.get_filter()
-        assert scenes.rel_state_err(x, xo, x0) < 1e-5 and scenes.rel_cov_err(P, Po) < 1e-5
+        scenes.check_filter(x, P, xo, Po, KIN_CHAIN_STATE_TOL, KIN_CHAIN_COV_TOL, f"scan {k}")
     eng.close()

@@ -179,11 +179,38 @@ def test_config1_literal_pin_2048_points():
         x, P, _, _ = o.get_filter()
         out.append((r["n_eff"], x, P))
     assert out[0][0] == out[1][0] > 0.9 * len(pts)
-    assert scenes.rel_state_err(out[1][1], out[0][1], x0) < 1e-9
-    assert scenes.rel_cov_err(out[1][2], out[0][2]) < 1e-9
+    scenes.check_filter(out[1][1], out[1][2], out[0][1], out[0][2], 8e-13, 7e-13)  # measured 8.4e-15 sd, 8.0e-15
     # the filter moved towards the true pose (Exp([2,-1,3]e-3), [0.02,-0.01,0.03]) where the plane constrains it
     d = lko.boxminus(out[0][1], x0)
     assert 1.2e-3 < d[0] < 2.2e-3 and -1.2e-3 < d[1] < -0.6e-3 and d[5] > 0
+
+
+def test_filter_comparison_catches_pose_block_errors():
+    """scenes.state_err / cov_err at the tolerances of the device's streaming tests, on the oracle's output for the inputs
+    of test_gpu_parity.py::test_streaming_buckets_static_map. There ~50 predicts make the imu_w / imu_a variances ~1e4
+    times the pose block's, which an error measured against P's largest entry cannot see past."""
+    import test_gpu_parity as tp
+    cfg, blob, scans = scenes.box_scene(batch=1, streaming=True, stream0=500)
+    pts, _, _ = synth.bucketize(scans[0], begin_time=100.0)
+    x0 = tp._moving_state(); P0 = abi.init_cov(1)
+    clk0 = np.zeros(1, abi.CLOCK_DTYPE); clk0["last_predict_time"] = 99.99; clk0["last_update_time"] = 99.985
+    runs = {}
+    for gain in (lko.GAIN_LITERAL, lko.GAIN_INFORMATION):
+        _, x, P, _, _ = tp._oracle_stream(cfg, blob, pts, 100.0, x0, P0, clk0, gain=gain)
+        runs[gain] = x, P.reshape(30, 30)
+    x, P = runs[lko.GAIN_INFORMATION]
+    assert np.abs(P).max() > 1e3 * np.abs(P[:6, :6]).max()
+    assert scenes.state_err(x, x, P) == 0.0 and scenes.cov_err(P, P) == 0.0
+    # the literal and the information form differ in arithmetic only
+    scenes.check_filter(*runs[lko.GAIN_LITERAL], x, P, tp.STATE_TOL, tp.COV_TOL)
+    bad = P.copy(); bad[:6, :6] *= 1.1  # the whole pose block of P 10 % off
+    e_block = scenes.cov_err(bad, P)
+    bad = P.copy(); bad[:3, 3:6] = 0.0; bad[3:6, :3] = 0.0  # attitude-position cross block dropped
+    e_cross = scenes.cov_err(bad, P)
+    step = lko.boxminus(x, x0)
+    e_step = scenes.state_err(lko.boxplus(x, np.r_[0.01 * step[:3], np.zeros(27)]), x, P)  # attitude step 1 % off
+    print(f"pose block x 1.1: {e_block!r}; cross block zeroed: {e_cross!r}; attitude step + 1 %: {e_step!r} sd")
+    assert e_block > tp.COV_TOL and e_cross > tp.COV_TOL and e_step > tp.STATE_TOL
 
 
 def test_noise_free_plane_gives_zero_innovation():

@@ -19,5 +19,5 @@ for iters in (1, 2, 3):
         for k, v in params.items(): eng.set_param(k, v)
         eng.map_upload(blob)
         out = eng.scan_update(x0, P0, Q, clk, pts, [0, len(pts)], [0.0], iters=iters)
-        res.append((params, int(out["n_eff"][0]), scenes.rel_state_err(out["x"], xo, x0)))
+        res.append((params, int(out["n_eff"][0]), scenes.state_err(out["x"], xo, Po)))
     print("iters", iters, "oracle", ro["n_eff"], res)

@@ -20,7 +20,7 @@ print("delta gpu", lko.boxminus(out["x"],x0)[:9]); print("delta cpu", lko.boxmin
 # oracle info-form update from GPU rows
 o2 = lko.Oracle(cfg); o2.set_filter(x0,P0,Q,None); o2.update_by_points(d["h"][m], d["z"][m], d["R"][m], gain_mode=1)
 x2,P2,_,_ = o2.get_filter(); print("delta cpu(gpu rows)", lko.boxminus(x2,x0)[:9])
-print("P err", scenes.rel_cov_err(out["P"][0],Po))
+print("P err", scenes.cov_err(out["P"][0],Po))
 import ctypes as C
 from legkilo_b200 import lib, _p
 part = np.zeros((8,32)); lib().lk_debug_read.argtypes=[C.c_void_p,C.c_int,C.c_void_p,C.c_size_t]
