@@ -81,10 +81,12 @@ __device__ __forceinline__ void ll_give_up(uint32_t* stall, uint32_t tag, uint32
 // keeps its words and is not loaded again (rows never change once published within an epoch), so a round loads only the
 // rows still missing. The level-1 poll of a group leader (<= 7 rows, one reader per row) reloads: keeping its words
 // across rounds costs the per-scan kernel spill stores and stack frame, and its rows have no other readers to slow down.
+// SPLIT < N: two sums in one poll, rows [0, SPLIT) returned and rows [SPLIT, n) in *hi, each from 0.0 in ascending order.
 // `rounds` receives the number of poll rounds. One full warp.
-template <int N, bool KEEP>
+template <int N, bool KEEP, int SPLIT = N>
 __device__ __forceinline__ double ll_sum_rows(const ulonglong2* rows, uint32_t r0, uint32_t n, uint32_t tag, int lane,
-                                              uint32_t* stall, uint32_t& rounds, double first = 0.0, bool have_first = false) {
+                                              uint32_t* stall, uint32_t& rounds, double first = 0.0, bool have_first = false,
+                                              double* hi = nullptr) {
     static_assert(N <= 32, "one bit per row");
     const ulonglong2* p = rows + (size_t)r0 * LL_ROW + lane;
     unsigned long long w0[N], w1[N];
@@ -134,11 +136,18 @@ __device__ __forceinline__ double ll_sum_rows(const ulonglong2* rows, uint32_t r
     rounds = spins;
     double s = 0.0;
 #pragma unroll
-    for (int k = 0; k < N; ++k)
+    for (int k = 0; k < SPLIT; ++k)
         if ((uint32_t)k < n) {
             const double v = (have_first && k == 0) ? first : __longlong_as_double((long long)((w0[k] & 0xffffffffull) | (w1[k] << 32)));
             s += v;
         }
+    if constexpr (SPLIT < N) {
+        double s2 = 0.0;
+#pragma unroll
+        for (int k = SPLIT; k < N; ++k)
+            if ((uint32_t)k < n) s2 += __longlong_as_double((long long)((w0[k] & 0xffffffffull) | (w1[k] << 32)));
+        *hi = s2;
+    }
     return s;
 }
 
@@ -219,18 +228,21 @@ __device__ __forceinline__ void ll_publish_row(const LLView& ll, uint32_t parity
 
 // The last exchange of a launch with finishers, the finisher side: the total of the n_chunks chunk rows in one hop, in
 // the grouped order of ll_allreduce (each group summed from 0.0 in ascending row order, then the group sums in ascending
-// order). Warp w sums groups w, w + NWARPS, ... into gs[g * 32 + lane] (LL_MAX_GROUPS * 32 doubles); result in
-// out[0..31]. All threads of the block call.
+// order). Warp w polls the group pairs w, w + NWARPS, ... (groups 2p and 2p + 1: up to 2 * LK_GROUP consecutive rows) in
+// one poll that keeps the rows it has seen, and stores the two group sums in gs[g * 32 + lane] (LL_MAX_GROUPS * 32
+// doubles); result in out[0..31]. All threads of the block call.
 template <int NWARPS>
 __device__ __forceinline__ void ll_sum_chunk_rows(const LLView& ll, uint32_t parity, uint32_t tag, uint32_t n_chunks, double* gs,
                                                   double* out) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const ulonglong2* crows = ll.chunk_rows + (size_t)parity * LL_MAX_CHUNKS * LL_ROW;
     const uint32_t n_groups = (n_chunks + LK_GROUP - 1) / LK_GROUP;
-    for (uint32_t g = (uint32_t)warp; g < n_groups; g += NWARPS) {
+    for (uint32_t g = 2u * (uint32_t)warp; g < n_groups; g += 2u * NWARPS) {
         uint32_t rounds;
-        gs[g * 32 + lane] = ll_sum_rows<LK_GROUP, false>(crows, g * LK_GROUP, min((uint32_t)LK_GROUP, n_chunks - g * LK_GROUP), tag,
-                                                         lane, ll.stall, rounds);
+        double hi;
+        gs[g * 32 + lane] = ll_sum_rows<2 * LK_GROUP, true, LK_GROUP>(crows, g * LK_GROUP, min(2u * LK_GROUP, n_chunks - g * LK_GROUP),
+                                                                       tag, lane, ll.stall, rounds, 0.0, false, &hi);
+        if (g + 1 < n_groups) gs[(g + 1) * 32 + lane] = hi;
     }
     __syncthreads();
     if (tid < 32) {
