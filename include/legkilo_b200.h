@@ -228,6 +228,26 @@ int lk_map_download(lk_handle h, void* blob, size_t capacity, size_t* bytes_out)
  * xyz_world = feats_down_world_ (float xyz, n*3), xyz_body = feats_down_body_ (lidar frame). */
 int lk_map_build(lk_handle h, const float* xyz_world, const float* xyz_body, size_t n,
                  const double rot[9], const double rot_cov[9], const double pos_cov[9]);
+/* KILO::process's first frame (KILO.cc:331-353): StateInitialByImu / ByKinImu::processing (state_initial.hpp:34-117),
+ * cloudLidarToWorld (KILO.cc:89-106) and VoxelMapManager::BuildVoxelMap (voxel_map.cc:287-334) in one call.
+ *  pts            : n_pts float4 (x, y, z, w) in the lidar frame, the raw (not down-sampled) cloud as lk_decode_pointcloud2
+ *                   writes it; only x, y, z go into the map
+ *  imu / kin      : the frame's inertial queue, exactly one non-NULL (imu_mode_only_), n_meas samples
+ *  x_inout        : grav = -mean_acc / |mean_acc| * gravity, bw = mean_gyr, rot = I; every other field is left as passed
+ *                   (lk_state_default for a fresh stream). The means follow the reference's recurrence: seeded with
+ *                   sample 0, then mean += (s - mean) / N over every sample, sample 0 included.
+ *  P_out[900]     : 1e-6 I;  clk_out: both times = end_time;  acc_norm_out: |mean_acc| (the acc_norm of later calls)
+ *  pts_world_out  : nullable, n_pts float4 (x_w, y_w, z_w, w): p_w = R (R_ext p + t_ext) + pos with R = I and the caller's
+ *                   pos, fp64 in the reference's summation order without FMA, rounded to float (bitwise the reference's)
+ * The map is built from those world points and the lidar points with rot = I, rot_cov = P[0:3,0:3], pos_cov = P[3:6,3:6],
+ * and replaces the handle's map as lk_map_build does (a failed pool allocation leaves the handle with no map).
+ * LK_ERR_NOT_READY (nothing written, the map untouched): n_pts == 0 or n_meas == 0 ("Data packet is not ready",
+ * KILO.cc:326-329). LK_ERR_INVALID_ARG: a NULL required argument, both imu and kin, or n_pts >= 2^31.
+ * LK_ERR_CAPACITY / LK_ERR_OUT_OF_MEMORY as lk_map_build. Outputs are written only on success. */
+int lk_first_frame(lk_handle h, lk_state* x_inout, double* P_out, lk_stream_clock* clk_out, double* acc_norm_out,
+                   const float* pts, uint32_t n_pts, double end_time,
+                   const lk_imu_meas* imu, const lk_kinimu_meas* kin, uint32_t n_meas, double gravity,
+                   float* pts_world_out);
 /* Step 4 of KILO::predictUpdatePoint (KILO.cc:216-231) without the filter: UpdateVoxelMap (voxel_map.cc:336-361) of
  * n_sets point sets, each placed at its own pose. Set s holds pts[set_offsets[s] .. set_offsets[s+1]) (float4, lidar frame,
  * the 4th component ignored) and is placed with rot[9s..] (row-major body->world), pos[3s..], rot_cov[9s..] and

@@ -322,6 +322,31 @@ int check_stall(lk_handle h) {
     return fail(h, LK_ERR_CUDA, msg);
 }
 
+// StateInitialByImu / ByKinImu::processing (state_initial.hpp:34-117): the running means seeded with sample 0, which the
+// loop then visits again with N = 1; acc / gyr at the same offsets in both sample types.
+template <class Meas>
+void state_initial(const Meas* m, uint32_t n, double gravity, lk_state* x, double* acc_norm) {
+    double ma[3], mw[3];
+    for (int k = 0; k < 3; ++k) {
+        ma[k] = m[0].acc[k];
+        mw[k] = m[0].gyr[k];
+    }
+    int N = 1;
+    for (uint32_t i = 0; i < n; ++i, ++N)
+        for (int k = 0; k < 3; ++k) {
+            ma[k] += (m[i].acc[k] - ma[k]) / N;
+            mw[k] += (m[i].gyr[k] - mw[k]) / N;
+        }
+    double s = 0.0;
+    for (int k = 0; k < 3; ++k) s += ma[k] * ma[k];
+    *acc_norm = std::sqrt(s);
+    for (int k = 0; k < 3; ++k) {
+        x->grav[k] = -ma[k] / *acc_norm * gravity;
+        x->bw[k] = mw[k];
+    }
+    for (int i = 0; i < 9; ++i) x->rot[i] = (i % 4 == 0) ? 1.0 : 0.0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -592,6 +617,48 @@ int lk_map_build(lk_handle h, const float* xyz_world, const float* xyz_body, siz
     std::string err;
     int rc = map_build_device(h->map, h->g, h->world.as<float>(), h->pts.as<float>(), (uint32_t)n, rot, rot_cov, pos_cov, s, err);
     return rc ? fail(h, rc, err) : LK_OK;
+}
+
+int lk_first_frame(lk_handle h, lk_state* x_inout, double* P_out, lk_stream_clock* clk_out, double* acc_norm_out,
+                   const float* pts, uint32_t n_pts, double end_time, const lk_imu_meas* imu, const lk_kinimu_meas* kin,
+                   uint32_t n_meas, double gravity, float* pts_world_out) {
+    if (!h || !x_inout || !P_out || !clk_out || !acc_norm_out || (n_pts && !pts))
+        return fail(h, LK_ERR_INVALID_ARG, "null argument");
+    if (imu && kin) return fail(h, LK_ERR_INVALID_ARG, "pass either imu or kin samples, not both (imu_mode_only_, KILO.cc:379)");
+    if (n_meas && !imu && !kin) return fail(h, LK_ERR_INVALID_ARG, "n_meas > 0 without samples");
+    if (n_pts >= (1u << 31)) return fail(h, LK_ERR_INVALID_ARG, "too many points for one build");
+    if (!n_pts || !n_meas) return fail(h, LK_ERR_NOT_READY, "data packet is not ready: empty cloud or inertial queue (KILO.cc:326-329)");
+    enter(h);
+    lk_state x = *x_inout;
+    double acc_norm = 0.0;
+    if (imu) state_initial(imu, n_meas, gravity, &x, &acc_norm);
+    else state_initial(kin, n_meas, gravity, &x, &acc_norm);
+    // P = 1e-6 I (state_initial.hpp:68); BuildVoxelMap takes rot = I and P's rotation / position blocks (KILO.cc:337)
+    const double C[9] = {1e-6, 0.0, 0.0, 0.0, 1e-6, 0.0, 0.0, 0.0, 1e-6};
+    cudaStream_t s = h->stream;
+    const size_t n = n_pts;
+    // h->pts = raw float4 | body xyz, h->world = world float4 | world xyz
+    LK_CUDA(h->err, h->pts.ensure(n * 28));
+    LK_CUDA(h->err, h->world.ensure(n * 28));
+    h->batch = 0;  // the staging buffers were borrowed
+    float4* d_in = h->pts.as<float4>();
+    float* d_body = reinterpret_cast<float*>(d_in + n);
+    float4* d_world4 = h->world.as<float4>();
+    float* d_world = reinterpret_cast<float*>(d_world4 + n);
+    LK_CUDA(h->err, cudaMemcpyAsync(d_in, pts, n * 16, cudaMemcpyHostToDevice, s));
+    launch_first_frame_points(h->g, d_in, (uint32_t)n, x.rot, x.pos, d_body, d_world, pts_world_out ? d_world4 : nullptr, s);
+    std::string err;
+    const int rc = map_build_device(h->map, h->g, d_world, d_body, (uint32_t)n, x.rot, C, C, s, err);
+    if (rc) return fail(h, rc, err);
+    if (pts_world_out) {
+        LK_CUDA(h->err, cudaMemcpyAsync(pts_world_out, d_world4, n * 16, cudaMemcpyDeviceToHost, s));
+        LK_CUDA(h->err, cudaStreamSynchronize(s));
+    }
+    *x_inout = x;
+    for (int i = 0; i < LK_DIM_STATE * LK_DIM_STATE; ++i) P_out[i] = (i % (LK_DIM_STATE + 1) == 0) ? 1e-6 : 0.0;
+    clk_out->last_predict_time = clk_out->last_update_time = end_time;  // KILO.cc:350-351
+    *acc_norm_out = acc_norm;
+    return LK_OK;
 }
 
 // ---- batch staging / run / fetch ----------------------------------------------------------------

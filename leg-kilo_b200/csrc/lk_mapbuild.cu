@@ -78,6 +78,37 @@ __global__ void k_build_points(const float* __restrict__ xyz_world, const float*
     recs[i] = p;
 }
 
+// KILO::cloudLidarToWorld (KILO.cc:89-106) over a raw float4 cloud, one load per point: the body and world xyz that
+// k_build_points reads, and the world float4 the node publishes (w copied as pointLidarToWorld copies the intensity).
+// p_i = R_ext p + t_ext, p_w = R p_i + pos, each product the reference's s = 0; s += a_k b_k (so 0 + -0.0 = +0.0), no FMA.
+__device__ __forceinline__ double row_dot(const double* r, double x, double y, double z) {
+    double s = __dadd_rn(0.0, __dmul_rn(r[0], x));
+    s = __dadd_rn(s, __dmul_rn(r[1], y));
+    return __dadd_rn(s, __dmul_rn(r[2], z));
+}
+
+struct WorldPose {
+    double Re[9], te[3];  // extrinsics
+    double R[9], p[3];    // body -> world
+};
+
+__global__ void k_first_frame_points(const float4* __restrict__ pts, uint32_t n, WorldPose wp, float* __restrict__ xyz_body,
+                                     float* __restrict__ xyz_world, float4* __restrict__ world4) {
+    uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const float4 q = pts[i];
+    const double x = q.x, y = q.y, z = q.z;
+    double pi[3], pw[3];
+#pragma unroll
+    for (int k = 0; k < 3; ++k) pi[k] = __dadd_rn(row_dot(wp.Re + 3 * k, x, y, z), wp.te[k]);
+#pragma unroll
+    for (int k = 0; k < 3; ++k) pw[k] = __dadd_rn(row_dot(wp.R + 3 * k, pi[0], pi[1], pi[2]), wp.p[k]);
+    const float wx = __double2float_rn(pw[0]), wy = __double2float_rn(pw[1]), wz = __double2float_rn(pw[2]);
+    xyz_body[3 * i] = q.x; xyz_body[3 * i + 1] = q.y; xyz_body[3 * i + 2] = q.z;
+    xyz_world[3 * i] = wx; xyz_world[3 * i + 1] = wy; xyz_world[3 * i + 2] = wz;
+    if (world4) world4[i] = make_float4(wx, wy, wz, q.w);
+}
+
 __global__ void k_gather_points(const DevPoint* __restrict__ recs, const uint32_t* __restrict__ idx, uint32_t n,
                                 DevPoint* out) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -230,6 +261,21 @@ int map_build_device(MapDevHost& mh, const Globals& g, const float* d_xyz_world,
         err = "map pools overflowed repeatedly";
     }
     return rc;
+}
+
+void launch_first_frame_points(const Globals& g, const float4* d_pts, uint32_t n, const double* rot, const double* pos,
+                               float* d_xyz_body, float* d_xyz_world, float4* d_world4, cudaStream_t s) {
+    if (!n) return;
+    WorldPose wp;
+    for (int i = 0; i < 9; ++i) {
+        wp.Re[i] = g.Re[i];
+        wp.R[i] = rot[i];
+    }
+    for (int i = 0; i < 3; ++i) {
+        wp.te[i] = g.te[i];
+        wp.p[i] = pos[i];
+    }
+    k_first_frame_points<<<(n + 255) / 256, 256, 0, s>>>(d_pts, n, wp, d_xyz_body, d_xyz_world, d_world4);
 }
 
 }  // namespace lk

@@ -58,6 +58,10 @@ class MapDevHost {
 // lk_mapbuild.cu
 int map_build_device(MapDevHost& mh, const Globals& g, const float* d_xyz_world, const float* d_xyz_body, uint32_t n,
                      const double* rot, const double* rot_cov, const double* pos_cov, cudaStream_t s, std::string& err);
+// cloudLidarToWorld (KILO.cc:89-106) of a raw float4 lidar cloud at pose (rot, pos): the body / world xyz map_build_device
+// takes, and the world float4 (x, y, z, input w) when d_world4 is not null.
+void launch_first_frame_points(const Globals& g, const float4* d_pts, uint32_t n, const double* rot, const double* pos,
+                               float* d_xyz_body, float* d_xyz_world, float4* d_world4, cudaStream_t s);
 // lk_insert.cu — UpdateVoxelMap for one bucket (scratch buffers owned by the caller). Returns the number of
 // launches (0 = nothing to do). world != null: the bucket's re-projected cloud is written too (the caller then
 // skips its own re-projection kernel). small_parity != null enables the two-launch path for buckets of up to

@@ -75,6 +75,33 @@ class Core {
         check(lk_map_build(h_, xyz_world, xyz_body, n, R.data(), Cr.data(), Cp.data()));
     }
 
+    // The first-frame branch of KILO::process (KILO.cc:331-353): StateInitial over the frame's inertial queue (exactly one of
+    // imu / kin non-empty), cloudLidarToWorld at the state's position and BuildVoxelMap, in one call. xyzw: the raw cloud as
+    // float4 (x, y, z, w), as lk_decode_pointcloud2 writes it; world_xyzw (optional) receives cloud_down_world_out.
+    // Returns false with nothing changed when the cloud or the queue is empty ("Data packet is not ready", KILO.cc:326-329).
+    template <class StateT>
+    bool firstFrame(StateT& state, StateCov& cov, double& last_predict_time, double& last_update_time, double& acc_norm,
+                    const std::vector<float>& xyzw, double end_time, const std::vector<lk_imu_meas>& imu,
+                    const std::vector<lk_kinimu_meas>& kin, double gravity, std::vector<float>* world_xyzw = nullptr) {
+        lk_state x = toAbi(state);
+        RowCov P;
+        lk_stream_clock clk{};
+        double an = 0.0;
+        if (world_xyzw) world_xyzw->resize(xyzw.size());
+        const int rc = lk_first_frame(h_, &x, P.data(), &clk, &an, xyzw.data(), (uint32_t)(xyzw.size() / 4), end_time,
+                                      imu.empty() ? nullptr : imu.data(), kin.empty() ? nullptr : kin.data(),
+                                      (uint32_t)(imu.empty() ? kin.size() : imu.size()), gravity,
+                                      world_xyzw ? world_xyzw->data() : nullptr);
+        if (rc == LK_ERR_NOT_READY) return false;
+        check(rc);
+        fromAbi(x, state);
+        cov = P;
+        last_predict_time = clk.last_predict_time;
+        last_update_time = clk.last_update_time;
+        acc_norm = an;  // acc_norm_ (KILO.cc:349)
+        return true;
+    }
+
     // The second lambda of KILO::process (KILO.cc:367-396) for one scan whose points are already in the
     // canonical (stable, ascending curvature) order. Exactly one of imu / kin may be non-empty.
     template <class StateT>

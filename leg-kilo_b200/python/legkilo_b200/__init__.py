@@ -50,6 +50,7 @@ def lib():
         L.lk_map_upload.argtypes = [vp, vp, C.c_size_t]
         L.lk_map_download.argtypes = [vp, vp, C.c_size_t, vp]
         L.lk_map_build.argtypes = [vp, vp, vp, C.c_size_t, vp, vp, vp]
+        L.lk_first_frame.argtypes = [vp, vp, vp, vp, vp, vp, u32, dbl, vp, vp, u32, dbl, vp]
         L.lk_map_insert.argtypes = [vp, u32, vp, vp, vp, vp, vp, vp]
         L.lk_map_stats.argtypes = [vp, vp]
         L.lk_map_slide.argtypes = [vp, vp, vp, vp]
@@ -182,6 +183,21 @@ class Engine:
         pos_cov = 1e-6 * np.eye(3) if pos_cov is None else np.ascontiguousarray(pos_cov, np.float64)
         self._chk(lib().lk_map_build(self.h, _p(xyz_world), _p(xyz_body), len(xyz_world), _p(R), _p(rot_cov),
                                      _p(pos_cov)))
+
+    def first_frame(self, x, pts, end_time, imu=None, kin=None, gravity=9.81, world=True):
+        """lk_first_frame: the first frame of KILO::process (KILO.cc:331-353) on a raw float32 [n, 4] lidar cloud and the
+        frame's inertial queue (exactly one of imu / kin): StateInitial, the world cloud at the prior's position and the
+        map build. Returns x, P [900], clk, acc_norm and the world cloud (float32 [n, 4], None when world is False)."""
+        x = np.array(x, abi.STATE_DTYPE, copy=True).reshape(1)
+        pts = np.ascontiguousarray(pts, np.float32).reshape(-1, 4)
+        imu = None if imu is None else np.ascontiguousarray(imu, abi.IMU_DTYPE)
+        kin = None if kin is None else np.ascontiguousarray(kin, abi.KINIMU_DTYPE)
+        nm = len(imu) if imu is not None else (len(kin) if kin is not None else 0)
+        P = np.zeros(900); clk = np.zeros(1, abi.CLOCK_DTYPE); acc_norm = C.c_double(0.0)
+        out = np.zeros((len(pts), 4), np.float32) if world else None
+        self._chk(lib().lk_first_frame(self.h, _p(x), _p(P), _p(clk), C.byref(acc_norm), _p(pts), len(pts), float(end_time),
+                                       _p(imu), _p(kin), nm, float(gravity), _p(out)))
+        return dict(x=x, P=P, clk=clk, acc_norm=acc_norm.value, world=out)
 
     def map_insert(self, pts, set_offsets, rot, pos, rot_cov, pos_cov):
         """lk_map_insert: UpdateVoxelMap of point sets at known poses. pts float32 [n, 4] (lidar frame), set_offsets
