@@ -263,6 +263,39 @@ int lk_first_frame(lk_handle h, lk_state* x_inout, double* P_out, lk_stream_cloc
  * to the window that overflowed, and some of that window's). A staged batch stays staged. */
 int lk_map_insert(lk_handle h, uint32_t n_sets, const float* pts, const uint32_t* set_offsets, const double* rot,
                   const double* pos, const double* rot_cov, const double* pos_cov);
+/* Record of one pose in lk_score_poses (LK_SCORE_STRIDE doubles): the sums the LiDAR update (KILO.cc:187-210) would form.
+ *   [LK_SCORE_A, +21)        upper triangle, row-major, of sum h^T h / R over the residual rows (h = [p_i x R^T n, n])
+ *   [LK_SCORE_B, +6)         sum h^T z / R
+ *   [LK_SCORE_SUM_R]         sum R
+ *   [LK_SCORE_COUNT]         number of residual rows (success_pts_size_out, KILO.cc:180)
+ *   [LK_SCORE_SUM_Z2R]       sum z^2 / R
+ *   the rest of the stride is 0. */
+#define LK_SCORE_A 0
+#define LK_SCORE_B 21
+#define LK_SCORE_SUM_R 27
+#define LK_SCORE_COUNT 28
+#define LK_SCORE_SUM_Z2R 29
+#define LK_SCORE_STRIDE 32
+/* n_poses candidate poses of n_sets point sets, scored against the handle's map. No filter, map or staged batch is touched.
+ * Set s = pts[set_offsets[s] .. set_offsets[s+1]) (float4, lidar frame, 4th component ignored). Pose m places set
+ * pose_set[m] with rot[9m..] (row-major body->world) and pos[3m..]. rot_cov / pos_cov (9 each, shared by every pose) are the
+ * theta / position blocks of P that enter the point variance and the gate, through their symmetric parts, as in
+ * lk_map_insert. sums_out[LK_SCORE_STRIDE m ..] receives pose m's record (LK_SCORE_*).
+ * Every point goes through the rows of KILO::predictUpdatePoint (KILO.cc:122-210) at that pose: transform, body
+ * covariance, voxel key, home voxel, then the one neighbour voxel, on the hot plane images (the form lk_debug_residuals
+ * evaluates with "debug_records" 0). A pose's record depends only on that pose and its set, not on the other poses of the
+ * call, their order or their number.
+ * LK_ERR_NOT_READY: the handle has no map. LK_ERR_INVALID_ARG: a NULL argument with n_poses > 0, set_offsets not monotone,
+ * pose_set[m] >= n_sets, or a non-finite entry of rot, pos, rot_cov or pos_cov. On any error nothing is written.
+ * n_poses == 0 does nothing.
+ * Runs on the device with one host synchronisation. Device memory, kept by the handle and grown to the largest call:
+ * 16 bytes per point, 488 bytes per pose, 32 bytes per (256-point chunk, tile of up to 16 poses of its set), and at most
+ * 64 MB of partial rows (256 bytes per pose and chunk of its set: the poses run in consecutive windows of at most that; a
+ * pose whose set alone has more than 262 144 chunks takes a window of its own). Page-locked staging: the larger of the
+ * per-pose / per-tile inputs and the records. */
+int lk_score_poses(lk_handle h, uint32_t n_sets, const float* pts, const uint32_t* set_offsets, uint32_t n_poses,
+                   const uint32_t* pose_set, const double* rot, const double* pos, const double* rot_cov,
+                   const double* pos_cov, double* sums_out);
 /* Map counters: out[0]=roots, out[1]=nodes, out[2]=retained points, out[3]=plane nodes. */
 int lk_map_stats(lk_handle h, uint64_t out[4]);
 /* VoxelMapManager::mapSliding + clearMemOutOfMap (voxel_map.cc:552-594; dead code in the reference, needed for unbounded

@@ -102,6 +102,10 @@ struct lk_context {
     // lk_map_insert: one window's points, chunk table + placements (mi_small, staged in h_mi), and insert scratch
     DevBuf mi_pts, mi_small, mi_ipts, mi_root, mi_touched, mi_counters, mi_list;
     PinnedBuf h_mi;
+    // lk_score_poses: points, items | sums | pose constants (staged in h_sp, which also receives the records), the
+    // partial rows of one window, the records
+    DevBuf sp_pts, sp_small, sp_partial, sp_out;
+    PinnedBuf h_sp;
     int trace_on = 0;
     uint32_t trace_seq = 0;  // fused launches traced since the trace was switched on or last read back
     int lane_cache = 1;
@@ -1174,6 +1178,19 @@ static int run_range_impl(lk_handle h, uint32_t first, uint32_t count, int iters
     return insert_finish(h, fused);
 }
 
+// The ScanConst of a pose given without a filter (lk_map_insert, lk_score_poses), as scan_const_from fills it from one: R, p
+// and the symmetric parts of the theta / position blocks of P (row-major 3 x 3 each).
+static void scan_const_at(const double* R, const double* p, const double* Pt, const double* Pp, ScanConst& sc) {
+    for (int i = 0; i < 9; ++i) sc.R[i] = R[i];
+    for (int i = 0; i < 3; ++i) sc.p[i] = p[i];
+    const int ut[6][2] = {{0, 0}, {0, 1}, {0, 2}, {1, 1}, {1, 2}, {2, 2}};
+    for (int q = 0; q < 6; ++q) {
+        const int i = ut[q][0], j = ut[q][1];
+        sc.Pth[q] = 0.5 * (Pt[i * 3 + j] + Pt[j * 3 + i]);
+        sc.Ppp[q] = 0.5 * (Pp[i * 3 + j] + Pp[j * 3 + i]);
+    }
+}
+
 // lk_map_insert runs its input through the slice-and-sort insert in windows of at most this many points (DESIGN §3.5):
 // per window, the headroom a streaming scan of as many points reserves, and scratch of a fixed size.
 constexpr uint32_t MAP_INSERT_WINDOW = 32768u;
@@ -1224,19 +1241,7 @@ int lk_map_insert(lk_handle h, uint32_t n_sets, const float* pts, const uint32_t
         for (uint32_t t = s; t < n_sets && set_offsets[t] < p1; ++t) {
             const uint64_t a = std::max<uint64_t>(set_offsets[t], p0), b = std::min<uint64_t>(set_offsets[t + 1], p1);
             if (a >= b) continue;
-            // ScanConst as scan_const_from fills it from a filter: R, p and the symmetric parts of the two P blocks
-            ScanConst& sc = hs[nsc];
-            const double* R = rot + 9 * (size_t)t;
-            const double* Pt = rot_cov + 9 * (size_t)t;
-            const double* Pp = pos_cov + 9 * (size_t)t;
-            for (int i = 0; i < 9; ++i) sc.R[i] = R[i];
-            for (int i = 0; i < 3; ++i) sc.p[i] = pos[3 * (size_t)t + i];
-            const int ut[6][2] = {{0, 0}, {0, 1}, {0, 2}, {1, 1}, {1, 2}, {2, 2}};
-            for (int q = 0; q < 6; ++q) {
-                const int i = ut[q][0], j = ut[q][1];
-                sc.Pth[q] = 0.5 * (Pt[i * 3 + j] + Pt[j * 3 + i]);
-                sc.Ppp[q] = 0.5 * (Pp[i * 3 + j] + Pp[j * 3 + i]);
-            }
+            scan_const_at(rot + 9 * (size_t)t, pos + 3 * (size_t)t, rot_cov + 9 * (size_t)t, pos_cov + 9 * (size_t)t, hs[nsc]);
             for (uint64_t q = a; q < b; q += 256) {
                 ChunkDesc& cd = hc[nc++];
                 cd.scan = nsc;
@@ -1258,6 +1263,121 @@ int lk_map_insert(lk_handle h, uint32_t n_sets, const float* pts, const uint32_t
         if (rc) return rc;
         p0 = p1;
     }
+    return LK_OK;
+}
+
+// lk_score_poses keeps at most this many partial rows (256 bytes each) in flight: poses past it run in the next window.
+constexpr uint32_t SCORE_WINDOW_ROWS = 1u << 18;  // 64 MB
+
+int lk_score_poses(lk_handle h, uint32_t n_sets, const float* pts, const uint32_t* set_offsets, uint32_t n_poses,
+                   const uint32_t* pose_set, const double* rot, const double* pos, const double* rot_cov,
+                   const double* pos_cov, double* sums_out) {
+    if (!h) return LK_ERR_INVALID_ARG;
+    if (n_poses == 0) return LK_OK;
+    if (!pts || !set_offsets || !pose_set || !rot || !pos || !rot_cov || !pos_cov || !sums_out)
+        return fail(h, LK_ERR_INVALID_ARG, "null argument");
+    for (uint32_t s = 0; s < n_sets; ++s)
+        if (set_offsets[s + 1] < set_offsets[s]) return fail(h, LK_ERR_INVALID_ARG, "set_offsets not monotone");
+    bool finite = true;
+    for (int i = 0; i < 9; ++i) finite = finite && std::isfinite(rot_cov[i]) && std::isfinite(pos_cov[i]);
+    for (uint32_t m = 0; m < n_poses; ++m) {
+        if (pose_set[m] >= n_sets) return fail(h, LK_ERR_INVALID_ARG, "pose_set names a set past n_sets");
+        for (int i = 0; i < 9; ++i) finite = finite && std::isfinite(rot[9 * (size_t)m + i]);
+        for (int i = 0; i < 3; ++i) finite = finite && std::isfinite(pos[3 * (size_t)m + i]);
+    }
+    if (!finite) return fail(h, LK_ERR_INVALID_ARG, "non-finite pose or covariance");
+    if (!h->map.ready()) return fail(h, LK_ERR_NOT_READY, "no map: call lk_map_upload or lk_map_build first");
+    enter(h);
+    cudaStream_t st = h->stream;
+    auto n_chunks = [&](uint32_t s) { return (set_offsets[s + 1] - set_offsets[s] + SCORE_CHUNK - 1) / SCORE_CHUNK; };
+
+    // the pose table in set order (the caller's order within a set), cut into tiles of consecutive poses of one set, and
+    // the tiles into windows of at most SCORE_WINDOW_ROWS partial rows (or one tile); item order: tile-major, so the blocks
+    // in flight together score one set at neighbouring poses, and touch neighbouring voxels
+    std::vector<uint32_t> first(n_sets + 1, 0), ord(n_poses);
+    for (uint32_t m = 0; m < n_poses; ++m) ++first[pose_set[m] + 1];
+    for (uint32_t s = 0; s < n_sets; ++s) first[s + 1] += first[s];
+    {
+        std::vector<uint32_t> fill(first.begin(), first.end() - 1);
+        for (uint32_t m = 0; m < n_poses; ++m) ord[fill[pose_set[m]]++] = m;
+    }
+    std::vector<ScoreItem> items;
+    std::vector<ScoreSum> sums(n_poses);
+    std::vector<uint32_t> win_items(1, 0), win_sums(1, 0);  // item / pose-table start of each window
+    uint32_t rows = 0;
+    for (uint32_t s = 0; s < n_sets; ++s) {
+        const uint32_t nc = n_chunks(s);
+        const uint32_t tile = std::max<uint32_t>(1, std::min<uint32_t>(SCORE_TILE, nc ? SCORE_WINDOW_ROWS / nc : SCORE_TILE));
+        for (uint32_t p0 = first[s]; p0 < first[s + 1]; p0 += tile) {
+            const uint32_t np = std::min(tile, first[s + 1] - p0);
+            if (rows > 0 && (uint64_t)rows + (uint64_t)np * nc > SCORE_WINDOW_ROWS) {
+                win_items.push_back((uint32_t)items.size());
+                win_sums.push_back(p0);
+                rows = 0;
+            }
+            for (uint32_t c = 0; c < nc; ++c) {
+                ScoreItem it;
+                it.start = set_offsets[s] - set_offsets[0] + c * SCORE_CHUNK;
+                it.count = std::min(SCORE_CHUNK, set_offsets[s + 1] - set_offsets[s] - c * SCORE_CHUNK);
+                it.pose0 = p0;
+                it.n_poses = np;
+                it.row0 = rows + c;
+                it.row_stride = nc;
+                it.pad[0] = it.pad[1] = 0;
+                items.push_back(it);
+            }
+            for (uint32_t k = 0; k < np; ++k) sums[p0 + k] = ScoreSum{rows + k * nc, nc, ord[p0 + k], 0};
+            rows += np * nc;
+        }
+    }
+    win_items.push_back((uint32_t)items.size());
+    win_sums.push_back(n_poses);
+    uint32_t max_rows = 0;
+    for (size_t w = 0; w + 1 < win_sums.size(); ++w)
+        for (uint32_t p = win_sums[w]; p < win_sums[w + 1]; ++p) max_rows = std::max(max_rows, sums[p].row0 + sums[p].n_rows);
+
+    // one packed H2D block: items | sums | ScanConst per pose (pose-table order)
+    const size_t o_sums = align256(std::max<size_t>(items.size(), 1) * sizeof(ScoreItem));
+    const size_t o_sc = o_sums + align256((size_t)n_poses * sizeof(ScoreSum));
+    const size_t small_bytes = o_sc + (size_t)n_poses * sizeof(ScanConst);
+    const size_t out_bytes = (size_t)n_poses * PARTIAL_STRIDE * 8;
+    const uint64_t n_pts = (uint64_t)set_offsets[n_sets] - set_offsets[0];
+    LK_CUDA(h->err, h->sp_pts.ensure(std::max<uint64_t>(n_pts, 1) * 16));
+    LK_CUDA(h->err, h->sp_small.ensure(small_bytes));
+    LK_CUDA(h->err, h->sp_partial.ensure((size_t)std::max<uint32_t>(max_rows, 1) * PARTIAL_STRIDE * 8));
+    LK_CUDA(h->err, h->sp_out.ensure(out_bytes));
+    LK_CUDA(h->err, h->h_sp.ensure(std::max(small_bytes, out_bytes)));
+    char* hb = (char*)h->h_sp.p;
+    std::memcpy(hb, items.data(), items.size() * sizeof(ScoreItem));
+    std::memcpy(hb + o_sums, sums.data(), (size_t)n_poses * sizeof(ScoreSum));
+    ScanConst* hs = reinterpret_cast<ScanConst*>(hb + o_sc);
+    for (uint32_t p = 0; p < n_poses; ++p) scan_const_at(rot + 9 * (size_t)ord[p], pos + 3 * (size_t)ord[p], rot_cov, pos_cov, hs[p]);
+    if (n_pts) LK_CUDA(h->err, cudaMemcpyAsync(h->sp_pts.p, pts + 4 * (size_t)set_offsets[0], n_pts * 16, cudaMemcpyHostToDevice, st));
+    LK_CUDA(h->err, cudaMemcpyAsync(h->sp_small.p, hb, small_bytes, cudaMemcpyHostToDevice, st));
+
+    ScoreArgs a;
+    std::memset(&a, 0, sizeof(a));
+    const MapDev md = h->map.dev();
+    a.pts = h->sp_pts.as<float4>();
+    a.items = h->sp_small.as<ScoreItem>();
+    a.sums = reinterpret_cast<const ScoreSum*>((char*)h->sp_small.p + o_sums);
+    a.sc = reinterpret_cast<const ScanConst*>((char*)h->sp_small.p + o_sc);
+    a.partial = h->sp_partial.as<double>();
+    a.out = h->sp_out.as<double>();
+    a.mv.slots = md.slots; a.mv.hash_mask = md.hash_mask; a.mv.nodes = md.nodes; a.mv.hot = md.hot;
+    a.g = h->g;
+    // the windows reuse the partial rows in stream order: window w + 1's blocks start after window w's sums are taken
+    for (size_t w = 0; w + 1 < win_items.size(); ++w) {
+        a.item_first = win_items[w];
+        a.sum_first = win_sums[w];
+        launch_score(a, win_items[w + 1] - win_items[w], win_sums[w + 1] - win_sums[w], st);
+        LK_CUDA(h->err, cudaGetLastError());
+    }
+    // the one host synchronisation: the staging block is reused for the records only after its H2D copy (same stream)
+    LK_CUDA(h->err, cudaMemcpyAsync(hb, h->sp_out.p, out_bytes, cudaMemcpyDeviceToHost, st));
+    LK_CUDA(h->err, cudaStreamSynchronize(st));
+    LK_CUDA(h->err, cudaGetLastError());
+    std::memcpy(sums_out, hb, out_bytes);
     return LK_OK;
 }
 

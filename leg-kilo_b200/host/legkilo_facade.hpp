@@ -128,6 +128,28 @@ class Core {
         return n_eff;  // success_pts_size_out
     }
 
+    // lk_score_poses: the sums the LiDAR update would form at each candidate pose, against the map, with no filter, map or
+    // staged batch touched. xyzw: float4 lidar-frame points, set s = points [set_offsets[s], set_offsets[s+1]); pose m places
+    // set pose_set[m] at (rot[m], pos[m]); rot_cov / pos_cov: the theta / position blocks of P shared by every pose.
+    // Returns LK_SCORE_STRIDE doubles per pose, laid out as LK_SCORE_* (count at LK_SCORE_COUNT).
+    std::vector<double> scorePoses(const std::vector<float>& xyzw, const std::vector<uint32_t>& set_offsets,
+                                   const std::vector<uint32_t>& pose_set, const std::vector<Mat3D>& rot,
+                                   const std::vector<Vec3D>& pos, const Mat3D& rot_cov, const Mat3D& pos_cov) {
+        const size_t n = pose_set.size();
+        if (rot.size() != n || pos.size() != n || set_offsets.empty())
+            throw std::invalid_argument("scorePoses: one rot / pos per pose, and set_offsets of n_sets + 1 entries");
+        std::vector<double> R(9 * n), p(3 * n), out(LK_SCORE_STRIDE * n);
+        for (size_t m = 0; m < n; ++m) {
+            RowMat3 Rm = rot[m];
+            std::memcpy(&R[9 * m], Rm.data(), 72);
+            std::memcpy(&p[3 * m], pos[m].data(), 24);
+        }
+        RowMat3 Cr = rot_cov, Cp = pos_cov;
+        check(lk_score_poses(h_, (uint32_t)(set_offsets.size() - 1), xyzw.data(), set_offsets.data(), (uint32_t)n,
+                             pose_set.data(), R.data(), p.data(), Cr.data(), Cp.data(), out.data()));
+        return out;
+    }
+
     // VoxelMapManager::mapSliding (voxel_map.cc:552-571): drop the root voxels that left the +-half_map_size window.
     bool mapSliding(const Vec3D& position_last, uint64_t* removed = nullptr) {
         int32_t slid = 0;

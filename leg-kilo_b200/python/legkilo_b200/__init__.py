@@ -52,6 +52,7 @@ def lib():
         L.lk_map_build.argtypes = [vp, vp, vp, C.c_size_t, vp, vp, vp]
         L.lk_first_frame.argtypes = [vp, vp, vp, vp, vp, vp, u32, dbl, vp, vp, u32, dbl, vp]
         L.lk_map_insert.argtypes = [vp, u32, vp, vp, vp, vp, vp, vp]
+        L.lk_score_poses.argtypes = [vp, u32, vp, vp, u32] + [vp] * 6
         L.lk_map_stats.argtypes = [vp, vp]
         L.lk_map_slide.argtypes = [vp, vp, vp, vp]
         L.lk_map_memory.argtypes = [vp, vp]
@@ -208,6 +209,28 @@ class Engine:
         rot, pos, rot_cov, pos_cov = (np.ascontiguousarray(a, np.float64).reshape(n_sets, k)
                                       for a, k in ((rot, 9), (pos, 3), (rot_cov, 9), (pos_cov, 9)))
         self._chk(lib().lk_map_insert(self.h, n_sets, _p(pts), _p(so), _p(rot), _p(pos), _p(rot_cov), _p(pos_cov)))
+
+    def score_poses(self, pts, set_offsets, pose_set, rot, pos, rot_cov, pos_cov):
+        """lk_score_poses: the sums of the LiDAR update at every candidate pose, against the map, touching nothing.
+        pts float32 [n, 4] (lidar frame), set_offsets [n_sets + 1]; per pose pose_set [n_poses], rot [n_poses, 3, 3],
+        pos [n_poses, 3]; rot_cov / pos_cov [3, 3] shared by every pose. Returns float64 [n_poses, 32], laid out as
+        abi.SCORE_* (A upper triangle | b | sum R | count | sum z^2 / R | 0 0)."""
+        pts = np.ascontiguousarray(pts, np.float32).reshape(-1, 4)
+        so = np.ascontiguousarray(set_offsets, np.uint32).reshape(-1)
+        if len(so) < 1:
+            raise ValueError("set_offsets needs n_sets + 1 entries")
+        if len(pts) < int(so[-1]):
+            raise ValueError(f"set_offsets ends at point {int(so[-1])}, pts has {len(pts)}")
+        ps = np.ascontiguousarray(pose_set, np.uint32).reshape(-1)
+        n_poses = len(ps)
+        rot = np.ascontiguousarray(rot, np.float64).reshape(n_poses, 9)
+        pos = np.ascontiguousarray(pos, np.float64).reshape(n_poses, 3)
+        rot_cov = np.ascontiguousarray(rot_cov, np.float64).reshape(9)
+        pos_cov = np.ascontiguousarray(pos_cov, np.float64).reshape(9)
+        out = np.zeros((n_poses, abi.SCORE_STRIDE))
+        self._chk(lib().lk_score_poses(self.h, len(so) - 1, _p(pts), _p(so), n_poses, _p(ps), _p(rot), _p(pos), _p(rot_cov),
+                                       _p(pos_cov), _p(out)))
+        return out
 
     def map_slide(self, position):
         """VoxelMapManager::mapSliding (voxel_map.cc:552-571). Returns (slid, removed root voxels)."""

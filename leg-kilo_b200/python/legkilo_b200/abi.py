@@ -112,6 +112,10 @@ MAP_POINT_DTYPE = np.dtype([("pw", "f8", (3,)), ("var", "f8", (6,))])
 assert MAP_HEADER_DTYPE.itemsize == 32 and MAP_ROOT_DTYPE.itemsize == 16
 assert MAP_NODE_DTYPE.itemsize == 256 and MAP_AUX_DTYPE.itemsize == 64 and MAP_POINT_DTYPE.itemsize == 72
 
+# lk_score_poses record (LK_SCORE_*): A = sum h^T h / R (upper triangle, 21) | b = sum h^T z / R (6) | sum R | count |
+# sum z^2 / R | 0 0
+SCORE_A, SCORE_B, SCORE_SUM_R, SCORE_COUNT, SCORE_SUM_Z2R, SCORE_STRIDE = 0, 21, 27, 28, 29, 32
+
 NODE_IS_PLANE, NODE_INIT_OCTO, NODE_UPDATE_ENABLE = 1, 2, 4
 NODE_LAYER_SHIFT, NODE_CHILDMASK_SHIFT = 8, 16
 
