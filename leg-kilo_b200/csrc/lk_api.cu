@@ -97,10 +97,9 @@ struct lk_context {
     PinnedBuf h_small_in, h_small_out;
     DevView chunks, stepinit, x_in, P_in, clk_in, Q, x, P, clk, n_eff, status;
     DevBuf dbg_ok, dbg_h, dbg_z, dbg_R, dbg_key, tmp, trace, bar;
-    DevBuf ins_pts, ins_root, ins_pend, ins_touched, ins_counters, ins_list;
-    uint64_t ins_pend_nodes = 0;
-    // lk_map_insert: one window's points, chunk table + placements (mi_small, staged in h_mi), and insert scratch
-    DevBuf mi_pts, mi_small, mi_ipts, mi_root, mi_touched, mi_counters, mi_list;
+    MapInserter inserter;  // UpdateVoxelMap: update_map runs and lk_map_insert
+    // lk_map_insert: one window's points, chunk table + placements (mi_small, staged in h_mi)
+    DevBuf mi_pts, mi_small;
     PinnedBuf h_mi;
     // lk_score_poses: points, items | sums | pose constants (staged in h_sp, which also receives the records), the
     // partial rows of one window, the records
@@ -952,11 +951,7 @@ static FusedArgs fused_args(lk_handle h, uint32_t first, int iters, bool insert,
     if (insert) {
         fa.insert = 1;
         fa.md = md;
-        fa.ipts = reinterpret_cast<DevPoint*>(h->ins_pts.p);
-        fa.iroot = h->ins_root.as<int>();
-        fa.pend = h->ins_pend.as<int>();
-        fa.touched = h->ins_touched.as<uint32_t>();
-        fa.ins_counters = h->ins_counters.as<uint32_t>() + 2;  // zeroed by run_range_impl, as for the two-launch insert
+        h->inserter.fused_scratch(fa);
     }
     return fa;
 }
@@ -1022,7 +1017,6 @@ static int run_kernels(lk_handle h, uint32_t first, uint32_t count, int iters, b
     const std::vector<StepInit>& tin = big ? h->h_initsL : h->h_inits;
     const ChunkDesc* d_chunks = big ? h->chunksL.as<ChunkDesc>() : h->chunks.as<ChunkDesc>();
     const StepInit* d_inits = big ? h->stepinitL.as<StepInit>() : h->stepinit.as<StepInit>();
-    uint32_t small_parity = 0;
     uint32_t mi = 0;
     if (mq) {  // the queue is applied BEFORE bucket 0 as well, so the filter is re-loaded here, not in the kernel
         LK_CUDA(h->err, cudaMemcpyAsync(h->x.as<lk_state>() + first, h->x_in.as<lk_state>() + first, sizeof(lk_state), cudaMemcpyDeviceToDevice, s));
@@ -1081,58 +1075,12 @@ static int run_kernels(lk_handle h, uint32_t first, uint32_t count, int iters, b
         }
         if (insert) {
             const StepInit& in = hin[first];
-            h->acc_launches += map_insert_bucket(h->map, h->g, h->pts.as<float4>(), d_chunks, c0, c1 - c0, in.pt_begin,
-                                                 in.pt_end - in.pt_begin, h->sc.as<ScanConst>(), h->step.as<ScanStep>(), h->ins_pts.p,
-                                                 h->ins_root.as<int>(), h->ins_pend.as<int>(), h->ins_touched.as<uint32_t>(),
-                                                 h->ins_counters.as<uint32_t>(), h->ins_list.as<uint32_t>(), s,
-                                                 insert_reprojects ? h->world.as<float4>() : nullptr,
-                                                 insert_reprojects ? &small_parity : nullptr);
+            h->acc_launches += h->inserter.bucket(h->map, h->g, h->pts.as<float4>(), d_chunks, c0, c1 - c0, in.pt_begin,
+                                                  in.pt_end - in.pt_begin, h->sc.as<ScanConst>(), h->step.as<ScanStep>(), s,
+                                                  insert_reprojects ? h->world.as<float4>() : nullptr);
         }
     }
     LK_CUDA(h->err, cudaGetLastError());
-    return LK_OK;
-}
-
-// Before an UpdateVoxelMap of up to n points (which may create the map): room for them in the pools, what earlier
-// launches freed made available (push_counters), and the per-root pending counts of the insert sized to the node pool.
-static int insert_headroom(lk_handle h, uint64_t n) {
-    cudaStream_t s = h->stream;
-    int rc = h->map.ready() ? h->map.sync_counters(s, h->err) : LK_OK;
-    // Worst case of UpdateVoxelMap per inserted point (lk_octree.cuh): a new root (1 node, one tile); per octree level one
-    // cut (8 nodes) whose children each get a tile — at most threshold + 1 of them hold a point when the cut fires; a
-    // tile is max_points_num + 2 slots (even). Reserving the bound makes a mid-insert overflow impossible: no point is
-    // ever dropped (the pools only grow when a scan could actually exceed them: 80 GB of HBM is the budget).
-    if (!rc) {
-        const Globals& g = h->g;
-        int thr = 0;
-        for (int l = 0; l < 5; ++l) thr = std::max(thr, g.layer_init_num[l]);
-        const uint64_t tile = (uint64_t)((g.max_points_num + 2 + 1) & ~1);
-        const uint64_t per_pt_nodes = 1 + 8ull * (uint64_t)std::max(g.max_layer, 0);
-        const uint64_t per_pt_slots = tile * (1 + (uint64_t)std::max(g.max_layer, 0) * (uint64_t)std::min(8, thr + 1)) + 2;
-        rc = h->map.ensure_headroom(n + 16, per_pt_nodes * n + 64, per_pt_slots * n + 64, s, h->err);
-    }
-    if (!rc) rc = h->map.push_counters(s, h->err);  // also makes what earlier launches freed available to this insert
-    if (rc) return rc;
-    if (h->ins_pend_nodes < h->map.node_cap) {
-        LK_CUDA(h->err, h->ins_pend.ensure((size_t)h->map.node_cap * 12));
-        LK_CUDA(h->err, cudaMemsetAsync(h->ins_pend.p, 0, h->ins_pend.cap, s));
-        h->ins_pend_nodes = h->map.node_cap;
-    }
-    return LK_OK;
-}
-
-// After the launches of an UpdateVoxelMap (fused: inside the per-scan kernel): wait for them, and report pools that ran
-// out (push_counters clears the flag).
-static int insert_finish(lk_handle h, bool fused) {
-    int rc = h->map.sync_counters(h->stream, h->err);  // also a sync
-    if (rc) return rc;
-    if (fused) {
-        rc = check_stall(h);
-        if (rc) return rc;
-    }
-    uint32_t ovf = 0;
-    LK_CUDA(h->err, cudaMemcpy(&ovf, h->map.dev().overflow, 4, cudaMemcpyDeviceToHost));
-    if (ovf) return fail(h, LK_ERR_CAPACITY, "map pools exhausted during UpdateVoxelMap (raise lk_map_reserve)");
     return LK_OK;
 }
 
@@ -1146,22 +1094,14 @@ static int run_range_impl(lk_handle h, uint32_t first, uint32_t count, int iters
     if (count == 0 || first + count > (uint32_t)h->batch) return fail(h, LK_ERR_INVALID_ARG, "scan range outside the staged batch");
     if (update_map && count != 1)
         return fail(h, LK_ERR_INVALID_ARG, "update_map inserts into this handle's map: run one scan (stream) per call");
-    cudaStream_t s = h->stream;
     uint32_t max_bucket = 0;
     if (update_map) {
-        int rc = insert_headroom(h, h->h_scan_pts[first]);
-        if (rc) return rc;
         for (uint32_t k = 0; k < h->n_steps; ++k) {
             const StepInit& in = h->h_inits[(size_t)k * h->batch + first];
             max_bucket = std::max(max_bucket, in.pt_end - in.pt_begin);
         }
-        const size_t mb = std::max<size_t>(max_bucket, 1);
-        LK_CUDA(h->err, h->ins_pts.ensure(mb * insert_point_bytes()));
-        LK_CUDA(h->err, h->ins_root.ensure(mb * 4));
-        LK_CUDA(h->err, h->ins_touched.ensure(mb * 4));
-        LK_CUDA(h->err, h->ins_list.ensure(2 * mb * 4));
-        LK_CUDA(h->err, h->ins_counters.ensure(64));
-        LK_CUDA(h->err, cudaMemsetAsync(h->ins_counters.p, 0, 64, s));
+        const int rc = h->inserter.begin(h->map, h->g, h->h_scan_pts[first], max_bucket, h->stream, h->err);
+        if (rc) return rc;
     }
     if (!h->map.ready()) return fail(h, LK_ERR_NOT_READY, "no map: call lk_map_upload or lk_map_build first");
     // update_map inside the persistent kernel: buckets of up to 4 096 points (the root-per-point scan of its insert phase)
@@ -1173,9 +1113,11 @@ static int run_range_impl(lk_handle h, uint32_t first, uint32_t count, int iters
         return fail(h, LK_ERR_CUDA, "batch staged by lk_scan_update for the per-scan kernel: re-stage it to run it another way");
     int rc = fused ? run_fused(h, first, iters, update_map, mq, timed) : run_kernels(h, first, count, iters, update_map, mq, timed);
     if (rc || !update_map) return rc;
-    // update_map: the caller observes a finished insert
+    // update_map: the caller observes a finished insert; a per-scan kernel that gave up waiting reports that, not the pools
     h->prev_fused = false;
-    return insert_finish(h, fused);
+    rc = h->map.sync_counters(h->stream, h->err);
+    if (!rc && fused) rc = check_stall(h);
+    return rc ? rc : h->inserter.finish(h->map, h->err);
 }
 
 // The ScanConst of a pose given without a filter (lk_map_insert, lk_score_poses), as scan_const_from fills it from one: R, p
@@ -1217,11 +1159,6 @@ int lk_map_insert(lk_handle h, uint32_t n_sets, const float* pts, const uint32_t
     const size_t sc_off = align256(((size_t)W / 256u + max_sets) * sizeof(ChunkDesc));
     const size_t small_bytes = sc_off + (size_t)max_sets * sizeof(ScanConst);
     LK_CUDA(h->err, h->mi_pts.ensure((size_t)W * 16));
-    LK_CUDA(h->err, h->mi_ipts.ensure((size_t)W * insert_point_bytes()));
-    LK_CUDA(h->err, h->mi_root.ensure((size_t)W * 4));
-    LK_CUDA(h->err, h->mi_touched.ensure((size_t)W * 4));
-    LK_CUDA(h->err, h->mi_list.ensure((size_t)2 * W * 4));
-    LK_CUDA(h->err, h->mi_counters.ensure(64));
     LK_CUDA(h->err, h->mi_small.ensure(small_bytes));
     LK_CUDA(h->err, h->h_mi.ensure(small_bytes));
     ChunkDesc* hc = reinterpret_cast<ChunkDesc*>(h->h_mi.p);
@@ -1233,7 +1170,7 @@ int lk_map_insert(lk_handle h, uint32_t n_sets, const float* pts, const uint32_t
     for (uint64_t p0 = set_offsets[0]; p0 < end;) {
         const uint64_t p1 = std::min<uint64_t>(end, p0 + W);
         const uint32_t n = (uint32_t)(p1 - p0);
-        int rc = insert_headroom(h, n);
+        int rc = h->inserter.begin(h->map, h->g, n, W, st, h->err);
         if (rc) return rc;
         // the window's chunks; ChunkDesc.scan = the set's row in the window's table of placements
         uint32_t nc = 0, nsc = 0;
@@ -1252,14 +1189,13 @@ int lk_map_insert(lk_handle h, uint32_t n_sets, const float* pts, const uint32_t
             ++nsc;
         }
         LK_CUDA(h->err, cudaMemcpyAsync(h->mi_pts.p, pts + 4 * p0, (size_t)n * 16, cudaMemcpyHostToDevice, st));
-        // (h_mi is free again: the previous window's insert_finish waited for its copies)
+        // (h_mi is free again: the previous window's sync_counters waited for its copies)
         LK_CUDA(h->err, cudaMemcpyAsync(h->mi_small.p, hc, (size_t)nc * sizeof(ChunkDesc), cudaMemcpyHostToDevice, st));
         LK_CUDA(h->err, cudaMemcpyAsync((char*)h->mi_small.p + sc_off, hs, (size_t)nsc * sizeof(ScanConst), cudaMemcpyHostToDevice, st));
-        map_insert_bucket(h->map, h->g, h->mi_pts.as<float4>(), dc, 0, nc, 0, n, ds, nullptr, h->mi_ipts.p,
-                          h->mi_root.as<int>(), h->ins_pend.as<int>(), h->mi_touched.as<uint32_t>(), h->mi_counters.as<uint32_t>(),
-                          h->mi_list.as<uint32_t>(), st);
+        h->inserter.bucket(h->map, h->g, h->mi_pts.as<float4>(), dc, 0, nc, 0, n, ds, nullptr, st);
         LK_CUDA(h->err, cudaGetLastError());
-        rc = insert_finish(h, false);
+        rc = h->map.sync_counters(st, h->err);
+        if (!rc) rc = h->inserter.finish(h->map, h->err);
         if (rc) return rc;
         p0 = p1;
     }

@@ -144,12 +144,43 @@ __global__ void __launch_bounds__(128) k_insert_p4_scan(const __grid_constant__ 
 
 }  // namespace
 
-// Scratch owned by the caller (lk_api): sized for the largest bucket.
-int map_insert_bucket(MapDevHost& mh, const Globals& g, const float4* pts, const ChunkDesc* chunks, uint32_t chunk_first,
-                      uint32_t n_chunks, uint32_t pt_begin, uint32_t n_pts, const ScanConst* sc, const ScanStep* step,
-                      void* ipts, int* iroot, int* pend, uint32_t* touched, uint32_t* counters, uint32_t* list,
-                      cudaStream_t s, float4* world, uint32_t* small_parity) {
+int MapInserter::begin(MapDevHost& mh, const Globals& g, uint64_t n, uint32_t max_bucket, cudaStream_t s, std::string& err) {
+    int rc = mh.ready() ? mh.sync_counters(s, err) : LK_OK;
+    // Worst case of UpdateVoxelMap per inserted point (lk_octree.cuh): a new root (1 node, one tile); per octree level one
+    // cut (8 nodes) whose children each get a tile — at most threshold + 1 of them hold a point when the cut fires.
+    // Reserving the bound makes a mid-insert overflow impossible: no point is ever dropped (the pools only grow when a
+    // scan could actually exceed them: 80 GB of HBM is the budget).
+    if (!rc) {
+        int thr = 0;
+        for (int l = 0; l < 5; ++l) thr = std::max(thr, g.layer_init_num[l]);
+        const uint64_t tile = mh.tile_slots;
+        const uint64_t per_pt_nodes = 1 + 8ull * (uint64_t)std::max(g.max_layer, 0);
+        const uint64_t per_pt_slots = tile * (1 + (uint64_t)std::max(g.max_layer, 0) * (uint64_t)std::min(8, thr + 1)) + 2;
+        rc = mh.ensure_headroom(n + 16, per_pt_nodes * n + 64, per_pt_slots * n + 64, s, err);
+    }
+    if (!rc) rc = mh.push_counters(s, err);  // also makes what earlier launches freed available to this insert
+    if (rc) return rc;
+    if (pend_nodes_ < mh.node_cap) {
+        LK_CUDA(err, pend_.ensure((size_t)mh.node_cap * 3 * sizeof(int)));
+        LK_CUDA(err, cudaMemsetAsync(pend_.p, 0, pend_.cap, s));
+        pend_nodes_ = mh.node_cap;
+    }
+    const size_t mb = std::max<uint32_t>(max_bucket, 1);
+    LK_CUDA(err, pts_.ensure(mb * sizeof(DevPoint)));
+    LK_CUDA(err, root_.ensure(mb * 4));
+    LK_CUDA(err, touched_.ensure(mb * 4));
+    LK_CUDA(err, list_.ensure(2 * mb * 4));
+    LK_CUDA(err, counters_.ensure(64));
+    LK_CUDA(err, cudaMemsetAsync(counters_.p, 0, 64, s));
+    parity_ = 0;
+    return LK_OK;
+}
+
+int MapInserter::bucket(const MapDevHost& mh, const Globals& g, const float4* pts, const ChunkDesc* chunks,
+                        uint32_t chunk_first, uint32_t n_chunks, uint32_t pt_begin, uint32_t n_pts, const ScanConst* sc,
+                        const ScanStep* step, cudaStream_t s, float4* world) {
     if (!n_pts || !n_chunks) return LK_OK;
+    uint32_t* counters = counters_.as<uint32_t>();
     InsertArgs a;
     a.md = mh.dev();
     a.g = g;
@@ -158,23 +189,22 @@ int map_insert_bucket(MapDevHost& mh, const Globals& g, const float4* pts, const
     a.chunk_first = chunk_first;
     a.sc = sc;
     a.step = step;
-    a.ipts = reinterpret_cast<DevPoint*>(ipts);
-    a.iroot = iroot;
+    a.ipts = pts_.as<DevPoint>();
+    a.iroot = root_.as<int>();
     a.pt_base = pt_begin;
-    a.pend = pend;
-    a.touched = touched;
+    a.pend = pend_.as<int>();
+    a.touched = touched_.as<uint32_t>();
     a.counters = counters;
-    a.list = list;
+    a.list = list_.as<uint32_t>();
     a.n_pts = n_pts;
     a.world = world;
     a.cslot = 0;
     const int wpb = 4;
-    if (small_parity && n_pts <= 4096u) {
-        // counters[2 + parity] is this bucket's n_touched; P4S zeroes the other one for the next bucket (the caller
-        // zeroed both before the first bucket of the scan)
+    if (world && n_pts <= 4096u) {
+        // counters[2 + parity] is this bucket's n_touched; P4S zeroes the other one for the next bucket (begin zeroed both)
         a.counters = counters + 2;
-        a.cslot = *small_parity;
-        *small_parity ^= 1u;
+        a.cslot = parity_;
+        parity_ ^= 1u;
         k_insert_p1<<<n_chunks, 256, 0, s>>>(a);
         k_insert_p4_scan<<<(n_pts + wpb - 1) / wpb, wpb * 32, wpb * sizeof(WarpTile), s>>>(a);
         return 2;
@@ -187,6 +217,19 @@ int map_insert_bucket(MapDevHost& mh, const Globals& g, const float4* pts, const
     return 5;
 }
 
-size_t insert_point_bytes() { return sizeof(DevPoint); }
+int MapInserter::finish(const MapDevHost& mh, std::string& err) const {
+    uint32_t ovf = 0;
+    LK_CUDA(err, cudaMemcpy(&ovf, mh.dev().overflow, 4, cudaMemcpyDeviceToHost));
+    if (ovf) err = "map pools exhausted during UpdateVoxelMap (raise lk_map_reserve)";
+    return ovf ? LK_ERR_CAPACITY : LK_OK;
+}
+
+void MapInserter::fused_scratch(FusedArgs& fa) const {
+    fa.ipts = pts_.as<DevPoint>();
+    fa.iroot = root_.as<int>();
+    fa.pend = pend_.as<int>();
+    fa.touched = touched_.as<uint32_t>();
+    fa.ins_counters = counters_.as<uint32_t>() + 2;
+}
 
 }  // namespace lk

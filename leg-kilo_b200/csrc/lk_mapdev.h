@@ -9,6 +9,7 @@
 namespace lk {
 
 struct DevPoint;
+struct FusedArgs;
 struct MapDev;
 
 class MapDevHost {
@@ -62,15 +63,29 @@ int map_build_device(MapDevHost& mh, const Globals& g, const float* d_xyz_world,
 // takes, and the world float4 (x, y, z, input w) when d_world4 is not null.
 void launch_first_frame_points(const Globals& g, const float4* d_pts, uint32_t n, const double* rot, const double* pos,
                                float* d_xyz_body, float* d_xyz_world, float4* d_world4, cudaStream_t s);
-// lk_insert.cu — UpdateVoxelMap for one bucket (scratch buffers owned by the caller). Returns the number of
-// launches (0 = nothing to do). world != null: the bucket's re-projected cloud is written too (the caller then
-// skips its own re-projection kernel). small_parity != null enables the two-launch path for buckets of up to
-// 4 096 points; the caller zeroes counters[2..3] and *small_parity before the first bucket of a scan.
-int map_insert_bucket(MapDevHost& mh, const Globals& g, const float4* pts, const ChunkDesc* chunks, uint32_t chunk_first,
-                      uint32_t n_chunks, uint32_t pt_begin, uint32_t n_pts, const ScanConst* sc, const ScanStep* step,
-                      void* ipts, int* iroot, int* pend, uint32_t* touched, uint32_t* counters, uint32_t* list,
-                      cudaStream_t s, float4* world = nullptr, uint32_t* small_parity = nullptr);
-size_t insert_point_bytes();
+// lk_insert.cu — UpdateVoxelMap (DESIGN §3.5), one per handle: shared by the streaming insert, the insert inside the
+// per-scan kernel and lk_map_insert. Its scratch is stream-ordered; no call keeps its contents.
+class MapInserter {
+   public:
+    // Before an UpdateVoxelMap of up to n points (which may create the map) in buckets of at most max_bucket points:
+    // room in the pools, what earlier launches freed made available (push_counters), pending counts for every node,
+    // scratch for one bucket, the touched-root counters cleared and the two-launch parity reset.
+    int begin(MapDevHost& mh, const Globals& g, uint64_t n, uint32_t max_bucket, cudaStream_t s, std::string& err);
+    // One bucket; returns the number of launches (0 = nothing to do). world != null: the bucket's re-projected cloud is
+    // written too (the caller then skips its own re-projection kernel), and buckets of up to 4 096 points take the
+    // two-launch path.
+    int bucket(const MapDevHost& mh, const Globals& g, const float4* pts, const ChunkDesc* chunks, uint32_t chunk_first,
+               uint32_t n_chunks, uint32_t pt_begin, uint32_t n_pts, const ScanConst* sc, const ScanStep* step,
+               cudaStream_t s, float4* world = nullptr);
+    // Once the stream is synchronised after the launches: report pools that ran out (push_counters clears the flag).
+    int finish(const MapDevHost& mh, std::string& err) const;
+    void fused_scratch(FusedArgs& fa) const;  // the scratch k_scan_fused<…, INS> inserts through
+
+   private:
+    DevBuf pts_, root_, touched_, list_, counters_, pend_;  // InsertArgs; counters: [2..3] are the two-launch path's
+    uint64_t pend_nodes_ = 0;  // nodes pend_ covers
+    uint32_t parity_ = 0;      // the two-launch counter of the next small bucket
+};
 // lk_mapio.cu
 int map_upload_blob(MapDevHost& mh, const Globals& g, const void* blob, size_t bytes, cudaStream_t s, std::string& err);
 int map_download_blob(MapDevHost& mh, void* blob, size_t capacity, size_t* bytes_out, cudaStream_t s, std::string& err);

@@ -9,7 +9,8 @@ windows that each run through the slice-and-sort insert.
 4. the hot plane images of inserted maps, through every kernel that reads them (tests/test_gpu_map_images.py: _probe);
 5. storage: freezes and cuts recycle tiles, a slide between calls recycles the window, repeated insertion of a static
    scene stops growing the pools;
-6. host behaviour: a staged batch survives the call, invalid arguments, n_sets = 0."""
+6. host behaviour: a staged batch survives the call, streaming inserts and the call share one handle's scratch, invalid
+   arguments, n_sets = 0."""
 import ctypes as C
 
 import numpy as np
@@ -236,6 +237,65 @@ def test_staged_batch_survives_an_insert():
         if x.dtype.names:
             x, y = x.view(np.float64), y.view(np.float64)
         np.testing.assert_array_equal(x, y, err_msg=k)
+
+
+@pytest.mark.parametrize("path", list(mi.INSERT_PATHS))
+def test_streaming_and_map_insert_share_scratch(path):
+    """update_map runs and lk_map_insert calls on one handle insert through the same scratch: small streaming buckets, a
+    call of three windows, one streaming bucket larger than a window (two VLP-16 revolutions: the scratch grows past the
+    window), a small call, small buckets again. A second handle with the same starting map replays every step as
+    lk_map_insert at the states and P blocks the first reported, and ends with the same map bitwise."""
+    cfg, blob, scans = scenes.box_scene(batch=5)
+    R, t = abi.extrinsics(cfg)
+    sc = synth.BoxScene(ground_half_extent=20.0)
+    Q = abi.process_cov_Q(cfg)
+    eng = _engine(cfg, blob)
+    fast, fused = mi.INSERT_PATHS[path]
+    eng.set_param("fast_insert", fast)
+    eng.set_param("fused_insert", fused)
+    x, P = abi.default_states(1), abi.init_cov(1)
+    clk = np.zeros(1, abi.CLOCK_DTYPE)
+    clk["last_predict_time"], clk["last_update_time"] = 9.99, 9.985
+    steps = []  # lk_map_insert arguments of every step, in order
+
+    def placement():
+        Pm = P[0].reshape(30, 30)
+        return [x["rot"][0].reshape(1, 3, 3), x["pos"][0].reshape(1, 3), Pm[None, :3, :3], Pm[None, 3:6, 3:6]]
+
+    def stream(p, t_bucket):
+        nonlocal x, P, clk
+        out = eng.scan_update(x, P, Q, clk, p, [0, len(p)], [t_bucket], iters=1, update_map=True)
+        x, P, clk = out["x"], out["P"], out["clk"]
+        steps.append([p, [0, len(p)]] + placement())
+
+    def insert(p, sizes):
+        args = [p, mic.offsets(sizes)] + [np.repeat(a, len(sizes), axis=0) for a in placement()]
+        eng.map_insert(*args)
+        steps.append(args)
+
+    def small_buckets(i, begin_time, n):
+        scan = sc.scan(rotvec=(0.0, 0.0, 0.01 * i), trans=(0.03 * i, -0.02 * i, 0.0), ext_R=R, ext_t=t, blind=cfg["blind"],
+                       stream=890 + i, streaming=True, **mm.LIDAR)
+        pts, offs, times = synth.bucketize(scan, begin_time=begin_time)
+        for b in range(n):
+            stream(pts[offs[b]:offs[b + 1]], times[b])
+        return times[n - 1]
+
+    t_last = small_buckets(0, 10.0, 4)
+    big = np.concatenate(scans[2:5])
+    assert len(big) > 2 * WINDOW, len(big)
+    insert(big, [len(s) for s in scans[2:5]])
+    two = np.concatenate(scans[:2])
+    assert len(two) > WINDOW, len(two)
+    stream(two, t_last + 0.002)
+    insert(scans[0][:3000], [1000, 2000])
+    small_buckets(1, 10.1, 4)
+
+    twin = _engine(cfg, blob)
+    for args in steps:
+        twin.map_insert(*args)
+    n = exact(eng.map_download(), twin.map_download())
+    print(f"[map insert] shared scratch ({path}): steps={len(steps)} nodes={n}")
 
 
 def _raw(eng, n_sets, pts, so, rot, pos, rc, pc):
