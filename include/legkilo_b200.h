@@ -296,6 +296,32 @@ int lk_map_insert(lk_handle h, uint32_t n_sets, const float* pts, const uint32_t
 int lk_score_poses(lk_handle h, uint32_t n_sets, const float* pts, const uint32_t* set_offsets, uint32_t n_poses,
                    const uint32_t* pose_set, const double* rot, const double* pos, const double* rot_cov,
                    const double* pos_cov, double* sums_out);
+/* n_poses candidate poses of n_sets point sets, each refined against the handle's map by iters steps of the LiDAR update
+ * with the pose's covariance held. No filter, map or staged batch is touched. The inputs are those of lk_score_poses, with
+ * the same meaning. One step of pose m:
+ *   1. its record (LK_SCORE_*) at the current pose, exactly as lk_score_poses forms it;
+ *   2. with P66 = blockdiag(sym(rot_cov), sym(pos_cov)): y = (I + A P66)^-1 b, delta = P66 y, i.e. K z of
+ *      ESKF::updateByPoints (eskf.cc:91-113) restricted to the pose, in information form, with the reference's N == 1 rule
+ *      (A and b scaled by sum R / (sum R + 1e-4) when the count is 1);
+ *   3. State::operator+= (eskf.cc:18-29): R <- R Exp(delta_theta), p <- p + delta_p. A count of 0, or a singular
+ *      I + A P66, gives a zero step.
+ * lk_batch_run(iters) re-applies the gain at every iterate with P held and updates P once, at the end. So the refined pose
+ * is the pose lk_batch_run(iters) gives for the one-bucket scan of the pose's set staged at that pose, when P's theta /
+ * position blocks are sym(rot_cov) / sym(pos_cov) with a zero cross block between them (no other entry of P reaches the
+ * pose) and the bucket time equals the clock (the predict is then the identity); the two differ only in the order in which
+ * the record's sums are added.
+ * rot_out[9m..] (row-major) / pos_out[3m..] receive pose m's refined pose; they may alias rot / pos. sums_out may be NULL;
+ * otherwise sums_out[LK_SCORE_STRIDE m ..] receives the record at the refined pose (one more scoring pass), bitwise what
+ * lk_score_poses returns for the refined poses with the same rot_cov / pos_cov.
+ * A pose's outputs depend only on that pose, its set, rot_cov, pos_cov and iters, not on the other poses of the call, their
+ * order or their number. No convergence test: every pose takes iters steps.
+ * LK_ERR_INVALID_ARG: iters < 1, NULL rot_out or pos_out with n_poses > 0, or an input lk_score_poses refuses;
+ * LK_ERR_NOT_READY: the handle has no map. On any error nothing is written. n_poses == 0 does nothing.
+ * Runs on the device with one host synchronisation, whatever iters. Device memory: the scratch of lk_score_poses, shared
+ * with it. Page-locked staging: the larger of the per-pose / per-tile inputs and the refined poses plus the records. */
+int lk_refine_poses(lk_handle h, uint32_t n_sets, const float* pts, const uint32_t* set_offsets, uint32_t n_poses,
+                    const uint32_t* pose_set, const double* rot, const double* pos, const double* rot_cov,
+                    const double* pos_cov, int iters, double* rot_out, double* pos_out, double* sums_out);
 /* Map counters: out[0]=roots, out[1]=nodes, out[2]=retained points, out[3]=plane nodes. */
 int lk_map_stats(lk_handle h, uint64_t out[4]);
 /* VoxelMapManager::mapSliding + clearMemOutOfMap (voxel_map.cc:552-594; dead code in the reference, needed for unbounded

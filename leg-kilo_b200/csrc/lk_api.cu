@@ -1205,12 +1205,11 @@ int lk_map_insert(lk_handle h, uint32_t n_sets, const float* pts, const uint32_t
 // lk_score_poses keeps at most this many partial rows (256 bytes each) in flight: poses past it run in the next window.
 constexpr uint32_t SCORE_WINDOW_ROWS = 1u << 18;  // 64 MB
 
-int lk_score_poses(lk_handle h, uint32_t n_sets, const float* pts, const uint32_t* set_offsets, uint32_t n_poses,
-                   const uint32_t* pose_set, const double* rot, const double* pos, const double* rot_cov,
-                   const double* pos_cov, double* sums_out) {
-    if (!h) return LK_ERR_INVALID_ARG;
-    if (n_poses == 0) return LK_OK;
-    if (!pts || !set_offsets || !pose_set || !rot || !pos || !rot_cov || !pos_cov || !sums_out)
+// The inputs lk_score_poses and lk_refine_poses share, checked as the header documents for both (n_poses > 0).
+static int score_check(lk_handle h, uint32_t n_sets, const float* pts, const uint32_t* set_offsets, uint32_t n_poses,
+                       const uint32_t* pose_set, const double* rot, const double* pos, const double* rot_cov,
+                       const double* pos_cov) {
+    if (!pts || !set_offsets || !pose_set || !rot || !pos || !rot_cov || !pos_cov)
         return fail(h, LK_ERR_INVALID_ARG, "null argument");
     for (uint32_t s = 0; s < n_sets; ++s)
         if (set_offsets[s + 1] < set_offsets[s]) return fail(h, LK_ERR_INVALID_ARG, "set_offsets not monotone");
@@ -1223,14 +1222,31 @@ int lk_score_poses(lk_handle h, uint32_t n_sets, const float* pts, const uint32_
     }
     if (!finite) return fail(h, LK_ERR_INVALID_ARG, "non-finite pose or covariance");
     if (!h->map.ready()) return fail(h, LK_ERR_NOT_READY, "no map: call lk_map_upload or lk_map_build first");
-    enter(h);
+    return LK_OK;
+}
+
+// What score_stage leaves for the launches: the kernels' arguments (one set for every window), the caller's pose index of
+// each pose-table entry, and the item / pose-table start of each window followed by the ends.
+struct ScorePlan {
+    ScoreArgs a;
+    std::vector<uint32_t> ord, win_items, win_sums;
+    size_t out_bytes;  // the records, n_poses * PARTIAL_STRIDE doubles
+};
+
+// The pose table of lk_score_poses / lk_refine_poses in set order (the caller's order within a set), cut into tiles of
+// consecutive poses of one set, and the tiles into windows of at most SCORE_WINDOW_ROWS partial rows (or one tile); item
+// order: tile-major, so the blocks in flight together score one set at neighbouring poses, and touch neighbouring voxels.
+// Sizes the handle's scratch, and queues the points and one packed block (items | sums | ScanConst per pose, pose-table
+// order) on its stream. The staging block h_sp holds at least back_bytes afterwards, for what the caller reads back into it
+// after the H2D copy (same stream).
+static int score_stage(lk_handle h, uint32_t n_sets, const float* pts, const uint32_t* set_offsets, uint32_t n_poses,
+                       const uint32_t* pose_set, const double* rot, const double* pos, const double* rot_cov,
+                       const double* pos_cov, size_t back_bytes, ScorePlan& sp) {
     cudaStream_t st = h->stream;
     auto n_chunks = [&](uint32_t s) { return (set_offsets[s + 1] - set_offsets[s] + SCORE_CHUNK - 1) / SCORE_CHUNK; };
-
-    // the pose table in set order (the caller's order within a set), cut into tiles of consecutive poses of one set, and
-    // the tiles into windows of at most SCORE_WINDOW_ROWS partial rows (or one tile); item order: tile-major, so the blocks
-    // in flight together score one set at neighbouring poses, and touch neighbouring voxels
-    std::vector<uint32_t> first(n_sets + 1, 0), ord(n_poses);
+    std::vector<uint32_t> first(n_sets + 1, 0);
+    std::vector<uint32_t>& ord = sp.ord;
+    ord.assign(n_poses, 0);
     for (uint32_t m = 0; m < n_poses; ++m) ++first[pose_set[m] + 1];
     for (uint32_t s = 0; s < n_sets; ++s) first[s + 1] += first[s];
     {
@@ -1239,7 +1255,9 @@ int lk_score_poses(lk_handle h, uint32_t n_sets, const float* pts, const uint32_
     }
     std::vector<ScoreItem> items;
     std::vector<ScoreSum> sums(n_poses);
-    std::vector<uint32_t> win_items(1, 0), win_sums(1, 0);  // item / pose-table start of each window
+    std::vector<uint32_t>&win_items = sp.win_items, &win_sums = sp.win_sums;
+    win_items.assign(1, 0);
+    win_sums.assign(1, 0);
     uint32_t rows = 0;
     for (uint32_t s = 0; s < n_sets; ++s) {
         const uint32_t nc = n_chunks(s);
@@ -1272,17 +1290,16 @@ int lk_score_poses(lk_handle h, uint32_t n_sets, const float* pts, const uint32_
     for (size_t w = 0; w + 1 < win_sums.size(); ++w)
         for (uint32_t p = win_sums[w]; p < win_sums[w + 1]; ++p) max_rows = std::max(max_rows, sums[p].row0 + sums[p].n_rows);
 
-    // one packed H2D block: items | sums | ScanConst per pose (pose-table order)
     const size_t o_sums = align256(std::max<size_t>(items.size(), 1) * sizeof(ScoreItem));
     const size_t o_sc = o_sums + align256((size_t)n_poses * sizeof(ScoreSum));
     const size_t small_bytes = o_sc + (size_t)n_poses * sizeof(ScanConst);
-    const size_t out_bytes = (size_t)n_poses * PARTIAL_STRIDE * 8;
+    sp.out_bytes = (size_t)n_poses * PARTIAL_STRIDE * 8;
     const uint64_t n_pts = (uint64_t)set_offsets[n_sets] - set_offsets[0];
     LK_CUDA(h->err, h->sp_pts.ensure(std::max<uint64_t>(n_pts, 1) * 16));
     LK_CUDA(h->err, h->sp_small.ensure(small_bytes));
     LK_CUDA(h->err, h->sp_partial.ensure((size_t)std::max<uint32_t>(max_rows, 1) * PARTIAL_STRIDE * 8));
-    LK_CUDA(h->err, h->sp_out.ensure(out_bytes));
-    LK_CUDA(h->err, h->h_sp.ensure(std::max(small_bytes, out_bytes)));
+    LK_CUDA(h->err, h->sp_out.ensure(sp.out_bytes));
+    LK_CUDA(h->err, h->h_sp.ensure(std::max(small_bytes, back_bytes)));
     char* hb = (char*)h->h_sp.p;
     std::memcpy(hb, items.data(), items.size() * sizeof(ScoreItem));
     std::memcpy(hb + o_sums, sums.data(), (size_t)n_poses * sizeof(ScoreSum));
@@ -1291,7 +1308,7 @@ int lk_score_poses(lk_handle h, uint32_t n_sets, const float* pts, const uint32_
     if (n_pts) LK_CUDA(h->err, cudaMemcpyAsync(h->sp_pts.p, pts + 4 * (size_t)set_offsets[0], n_pts * 16, cudaMemcpyHostToDevice, st));
     LK_CUDA(h->err, cudaMemcpyAsync(h->sp_small.p, hb, small_bytes, cudaMemcpyHostToDevice, st));
 
-    ScoreArgs a;
+    ScoreArgs& a = sp.a;
     std::memset(&a, 0, sizeof(a));
     const MapDev md = h->map.dev();
     a.pts = h->sp_pts.as<float4>();
@@ -1302,18 +1319,88 @@ int lk_score_poses(lk_handle h, uint32_t n_sets, const float* pts, const uint32_
     a.out = h->sp_out.as<double>();
     a.mv.slots = md.slots; a.mv.hash_mask = md.hash_mask; a.mv.nodes = md.nodes; a.mv.hot = md.hot;
     a.g = h->g;
+    return LK_OK;
+}
+
+// Window w of a plan: its sums (and k_score_sum's pose-table start) in a, and its item / pose counts.
+static void score_window(ScorePlan& sp, size_t w, uint32_t& n_items, uint32_t& n_sums) {
+    sp.a.item_first = sp.win_items[w];
+    sp.a.sum_first = sp.win_sums[w];
+    n_items = sp.win_items[w + 1] - sp.win_items[w];
+    n_sums = sp.win_sums[w + 1] - sp.win_sums[w];
+}
+
+int lk_score_poses(lk_handle h, uint32_t n_sets, const float* pts, const uint32_t* set_offsets, uint32_t n_poses,
+                   const uint32_t* pose_set, const double* rot, const double* pos, const double* rot_cov,
+                   const double* pos_cov, double* sums_out) {
+    if (!h) return LK_ERR_INVALID_ARG;
+    if (n_poses == 0) return LK_OK;
+    if (!sums_out) return fail(h, LK_ERR_INVALID_ARG, "null argument");
+    if (int rc = score_check(h, n_sets, pts, set_offsets, n_poses, pose_set, rot, pos, rot_cov, pos_cov)) return rc;
+    enter(h);
+    cudaStream_t st = h->stream;
+    ScorePlan sp;
+    if (int rc = score_stage(h, n_sets, pts, set_offsets, n_poses, pose_set, rot, pos, rot_cov, pos_cov,
+                             (size_t)n_poses * PARTIAL_STRIDE * 8, sp))
+        return rc;
     // the windows reuse the partial rows in stream order: window w + 1's blocks start after window w's sums are taken
-    for (size_t w = 0; w + 1 < win_items.size(); ++w) {
-        a.item_first = win_items[w];
-        a.sum_first = win_sums[w];
-        launch_score(a, win_items[w + 1] - win_items[w], win_sums[w + 1] - win_sums[w], st);
+    for (size_t w = 0; w + 1 < sp.win_items.size(); ++w) {
+        uint32_t n_items, n_sums;
+        score_window(sp, w, n_items, n_sums);
+        launch_score(sp.a, n_items, n_sums, st);
         LK_CUDA(h->err, cudaGetLastError());
     }
     // the one host synchronisation: the staging block is reused for the records only after its H2D copy (same stream)
-    LK_CUDA(h->err, cudaMemcpyAsync(hb, h->sp_out.p, out_bytes, cudaMemcpyDeviceToHost, st));
+    char* hb = (char*)h->h_sp.p;
+    LK_CUDA(h->err, cudaMemcpyAsync(hb, h->sp_out.p, sp.out_bytes, cudaMemcpyDeviceToHost, st));
     LK_CUDA(h->err, cudaStreamSynchronize(st));
     LK_CUDA(h->err, cudaGetLastError());
-    std::memcpy(sums_out, hb, out_bytes);
+    std::memcpy(sums_out, hb, sp.out_bytes);
+    return LK_OK;
+}
+
+int lk_refine_poses(lk_handle h, uint32_t n_sets, const float* pts, const uint32_t* set_offsets, uint32_t n_poses,
+                    const uint32_t* pose_set, const double* rot, const double* pos, const double* rot_cov,
+                    const double* pos_cov, int iters, double* rot_out, double* pos_out, double* sums_out) {
+    if (!h) return LK_ERR_INVALID_ARG;
+    if (n_poses == 0) return LK_OK;
+    if (!rot_out || !pos_out) return fail(h, LK_ERR_INVALID_ARG, "null argument");
+    if (iters < 1) return fail(h, LK_ERR_INVALID_ARG, "iters < 1");
+    if (int rc = score_check(h, n_sets, pts, set_offsets, n_poses, pose_set, rot, pos, rot_cov, pos_cov)) return rc;
+    enter(h);
+    cudaStream_t st = h->stream;
+    // read back into the staging block: the ScanConst of every pose (pose-table order), then the records if asked for
+    const size_t sc_bytes = (size_t)n_poses * sizeof(ScanConst), o_rec = align256(sc_bytes);
+    ScorePlan sp;
+    if (int rc = score_stage(h, n_sets, pts, set_offsets, n_poses, pose_set, rot, pos, rot_cov, pos_cov,
+                             o_rec + (sums_out ? (size_t)n_poses * PARTIAL_STRIDE * 8 : 0), sp))
+        return rc;
+    // the pose constants the items read are stepped in place: k_score takes them const, k_refine_step writable
+    ScanConst* sc = const_cast<ScanConst*>(sp.a.sc);
+    // window by window, every step of its poses, then (with sums_out) their records at the refined poses; the windows
+    // reuse the partial rows in stream order, and no launch waits for the host
+    for (size_t w = 0; w + 1 < sp.win_items.size(); ++w) {
+        uint32_t n_items, n_sums;
+        score_window(sp, w, n_items, n_sums);
+        for (int it = 0; it < iters; ++it) {
+            launch_score(sp.a, n_items, n_sums, st);
+            launch_refine_step(sp.a, sc, n_sums, st);
+        }
+        if (sums_out) launch_score(sp.a, n_items, n_sums, st);
+        LK_CUDA(h->err, cudaGetLastError());
+    }
+    // the one host synchronisation: the staging block is reused only after its H2D copy (same stream)
+    char* hb = (char*)h->h_sp.p;
+    LK_CUDA(h->err, cudaMemcpyAsync(hb, sc, sc_bytes, cudaMemcpyDeviceToHost, st));
+    if (sums_out) LK_CUDA(h->err, cudaMemcpyAsync(hb + o_rec, h->sp_out.p, sp.out_bytes, cudaMemcpyDeviceToHost, st));
+    LK_CUDA(h->err, cudaStreamSynchronize(st));
+    LK_CUDA(h->err, cudaGetLastError());
+    const ScanConst* hs = reinterpret_cast<const ScanConst*>(hb);
+    for (uint32_t p = 0; p < n_poses; ++p) {
+        std::memcpy(rot_out + 9 * (size_t)sp.ord[p], hs[p].R, sizeof(hs[p].R));
+        std::memcpy(pos_out + 3 * (size_t)sp.ord[p], hs[p].p, sizeof(hs[p].p));
+    }
+    if (sums_out) std::memcpy(sums_out, hb + o_rec, sp.out_bytes);
     return LK_OK;
 }
 

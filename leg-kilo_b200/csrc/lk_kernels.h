@@ -128,6 +128,9 @@ struct ScoreArgs {
     Globals g;
 };
 void launch_score(const ScoreArgs& a, uint32_t n_items, uint32_t n_sums, cudaStream_t s);
+// lk_refine_poses: one pose step (k_refine_step) for poses [sum_first, sum_first + n_sums) of the pose table, from the
+// records a.out holds at their current poses; the new R / p are written into sc, the same buffer as a.sc.
+void launch_refine_step(const ScoreArgs& a, ScanConst* sc, uint32_t n_sums, cudaStream_t s);
 
 // ---- fused per-scan persistent kernel (lk_fused.cu) -------------------------------------------
 constexpr int FUSED_INLINE_STEPS = 64;

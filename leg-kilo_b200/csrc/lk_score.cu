@@ -1,5 +1,6 @@
 // lk_score.cu — lk_score_poses: the sums the LiDAR update would form, at many candidate poses of each point set, against a
-// map that stays fixed for the call. No filter is read or written and nothing is solved.
+// map that stays fixed for the call; and lk_refine_poses, which steps each pose from those sums. No filter is read or
+// written.
 //
 // k_score: one block per (256-point chunk of a set, tile of up to SCORE_TILE of that set's poses). The block loads its chunk
 // once and forms what does not depend on the pose once (lk_point.cuh: body_point, kept in the lane's LaneCache); then, pose
@@ -11,6 +12,10 @@
 //
 // k_score_sum: one block per pose, its set's partial rows summed in ascending groups (block_sum_partials), so the record of
 // a pose depends only on that pose and its set.
+//
+// k_refine_step (lk_refine_poses): one warp per pose, one pose step from the pose's record: the information-form solve of
+// block_solve_state (its column assembly, warp_solve6) with the pose's P66 held, and State::operator+= on R and p, written into
+// the pose's ScanConst in place. Steps chain on the device: k_score, k_score_sum, k_refine_step, k_score, ...
 #include "lk_kernels.h"
 #include "lk_pass.cuh"
 #include "lk_solve.cuh"
@@ -26,6 +31,7 @@ namespace {
 constexpr int BLOCK = SCORE_CHUNK;  // one point per thread per pass
 constexpr int WARPS = BLOCK / 32;
 constexpr int SUM_THREADS = 128;
+constexpr int REFINE_THREADS = 128;  // four poses per block, one per warp
 
 __global__ void __launch_bounds__(BLOCK, 1) k_score(const __grid_constant__ ScoreArgs a) {
     extern __shared__ __align__(16) unsigned char s_raw[];
@@ -62,6 +68,74 @@ __global__ void __launch_bounds__(SUM_THREADS) k_score_sum(const __grid_constant
     if (threadIdx.x < 32) a.out[(size_t)ss.pose * PARTIAL_STRIDE + threadIdx.x] = s_out[threadIdx.x];
 }
 
+// Entry (i, j) of P66 = blockdiag(Pth, Ppp) from the packed upper triangles (xx xy xz yy yz zz); the cross blocks are 0.
+__device__ __forceinline__ double p66_entry(const ScanConst* sc, int i, int j) {
+    if ((i < 3) != (j < 3)) return 0.0;
+    const int o = i < 3 ? 0 : 3, r = min(i, j) - o, c = max(i, j) - o;
+    return (i < 3 ? sc->Pth : sc->Ppp)[r * 3 - r * (r - 1) / 2 + (c - r)];
+}
+
+// One step of one pose per warp: ESKF::updateByPoints' K z (eskf.cc:91-113) restricted to the pose, with P66 held, in the
+// information form of block_solve_state: y = (I + A P66)^-1 b from the pose's record (the sums at its current pose),
+// delta = P66 y, then State::operator+= (eskf.cc:18-29): R <- R Exp(delta_theta), p <- p + delta_p, written back into the
+// pose's ScanConst for the next k_score. A count of 0 leaves the pose untouched; a singular M gives a zero step, as in
+// block_solve_state.
+__global__ void __launch_bounds__(REFINE_THREADS) k_refine_step(const __grid_constant__ ScoreArgs a, ScanConst* sc, uint32_t n) {
+    const int lane = threadIdx.x & 31;
+    const uint32_t w = blockIdx.x * (REFINE_THREADS / 32) + (threadIdx.x >> 5);
+    if (w >= n) return;  // warp-uniform
+    const uint32_t pose = a.sum_first + w;
+    const double* acc = a.out + (size_t)a.sums[pose].pose * PARTIAL_STRIDE;
+    if (!(acc[ACC_CNT] > 0.5)) return;
+    ScanConst* s = sc + pose;
+    // N == 1 adds 1e-4 to S (eskf.cc:100)  <=>  weights scale by R / (R + 1e-4)
+    const double scale = (acc[ACC_CNT] < 1.5) ? acc[ACC_SUMR] / (acc[ACC_SUMR] + 0.0001) : 1.0;
+    // Pc: column `lane` of P66 (lanes 0..5), which is also its row: P66 is symmetric
+    double Pc[6];
+#pragma unroll
+    for (int k = 0; k < 6; ++k) Pc[k] = p66_entry(s, k, lane < 6 ? lane : 0);
+    // columns of [M | b | A], M = I + A P66, one per lane (0..12), formed as block_solve_state forms them
+    double col[6];
+#pragma unroll
+    for (int i = 0; i < 6; ++i) {
+        double ar[6];
+#pragma unroll
+        for (int k = 0; k < 6; ++k) {
+            const int r = i < k ? i : k, c = i < k ? k : i;
+            ar[k] = acc[r * 6 - r * (r - 1) / 2 + (c - r)] * scale;
+        }
+        double m = (i == lane) ? 1.0 : 0.0;
+#pragma unroll
+        for (int k = 0; k < 6; ++k) m += ar[k] * Pc[k];
+        double asel = ar[0];
+#pragma unroll
+        for (int t = 1; t < 6; ++t) asel = (lane - 7 == t) ? ar[t] : asel;
+        const double bsel = acc[ACC_B + i] * scale;
+        col[i] = lane < 6 ? m : (lane == 6 ? bsel : (lane < 13 ? asel : 0.0));
+    }
+    const bool ok = warp_solve6(col, lane);
+    double d = 0.0;
+#pragma unroll
+    for (int k = 0; k < 6; ++k) d += Pc[k] * __shfl_sync(0xffffffffu, ok ? col[k] : 0.0, 6);
+    const double d0 = __shfl_sync(0xffffffffu, d, 0), d1 = __shfl_sync(0xffffffffu, d, 1),
+                 d2 = __shfl_sync(0xffffffffu, d, 2);
+    const double dp = __shfl_sync(0xffffffffu, d, (lane + 26) & 31);  // lanes 9..11: delta_p from lanes 3..5
+    double rv = 0.0;
+    if (lane < 9) {
+        double E[9];
+        so3_exp3(d0, d1, d2, E);
+        // column j of E picked with compile-time indices (E indexed at run time would live in local memory)
+        const int i = lane / 3, j = lane % 3;
+        const double e0 = j == 0 ? E[0] : (j == 1 ? E[1] : E[2]);
+        const double e1 = j == 0 ? E[3] : (j == 1 ? E[4] : E[5]);
+        const double e2 = j == 0 ? E[6] : (j == 1 ? E[7] : E[8]);
+        rv = s->R[i * 3] * e0 + s->R[i * 3 + 1] * e1 + s->R[i * 3 + 2] * e2;
+    }
+    __syncwarp();
+    if (lane < 9) s->R[lane] = rv;
+    else if (lane < 12) s->p[lane - 9] += dp;
+}
+
 }  // namespace
 
 void launch_score(const ScoreArgs& a, uint32_t n_items, uint32_t n_sums, cudaStream_t s) {
@@ -70,6 +144,11 @@ void launch_score(const ScoreArgs& a, uint32_t n_items, uint32_t n_sums, cudaStr
     if (once.first()) cudaFuncSetAttribute(k_score, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (n_items) k_score<<<n_items, BLOCK, smem, s>>>(a);
     if (n_sums) k_score_sum<<<n_sums, SUM_THREADS, 0, s>>>(a);
+}
+
+void launch_refine_step(const ScoreArgs& a, ScanConst* sc, uint32_t n_sums, cudaStream_t s) {
+    constexpr uint32_t per_block = REFINE_THREADS / 32;
+    if (n_sums) k_refine_step<<<(n_sums + per_block - 1) / per_block, REFINE_THREADS, 0, s>>>(a, sc, n_sums);
 }
 
 }  // namespace lk

@@ -150,6 +150,32 @@ class Core {
         return out;
     }
 
+    // lk_refine_poses: each candidate pose refined in place by `iters` steps of the LiDAR update with the theta / position
+    // blocks of P held at rot_cov / pos_cov, against the map, with no filter, map or staged batch touched. Inputs as
+    // scorePoses. Returns the records at the refined poses (LK_SCORE_STRIDE doubles per pose, laid out as LK_SCORE_*).
+    std::vector<double> refinePoses(const std::vector<float>& xyzw, const std::vector<uint32_t>& set_offsets,
+                                    const std::vector<uint32_t>& pose_set, std::vector<Mat3D>& rot, std::vector<Vec3D>& pos,
+                                    const Mat3D& rot_cov, const Mat3D& pos_cov, int iters) {
+        const size_t n = pose_set.size();
+        if (rot.size() != n || pos.size() != n || set_offsets.empty())
+            throw std::invalid_argument("refinePoses: one rot / pos per pose, and set_offsets of n_sets + 1 entries");
+        std::vector<double> R(9 * n), p(3 * n), out(LK_SCORE_STRIDE * n);
+        for (size_t m = 0; m < n; ++m) {
+            RowMat3 Rm = rot[m];
+            std::memcpy(&R[9 * m], Rm.data(), 72);
+            std::memcpy(&p[3 * m], pos[m].data(), 24);
+        }
+        RowMat3 Cr = rot_cov, Cp = pos_cov;
+        check(lk_refine_poses(h_, (uint32_t)(set_offsets.size() - 1), xyzw.data(), set_offsets.data(), (uint32_t)n,
+                              pose_set.data(), R.data(), p.data(), Cr.data(), Cp.data(), iters, R.data(), p.data(),
+                              out.data()));
+        for (size_t m = 0; m < n; ++m) {
+            rot[m] = Eigen::Map<const RowMat3>(&R[9 * m]);
+            pos[m] = Eigen::Map<const Vec3D>(&p[3 * m]);
+        }
+        return out;
+    }
+
     // VoxelMapManager::mapSliding (voxel_map.cc:552-571): drop the root voxels that left the +-half_map_size window.
     bool mapSliding(const Vec3D& position_last, uint64_t* removed = nullptr) {
         int32_t slid = 0;

@@ -53,6 +53,7 @@ def lib():
         L.lk_first_frame.argtypes = [vp, vp, vp, vp, vp, vp, u32, dbl, vp, vp, u32, dbl, vp]
         L.lk_map_insert.argtypes = [vp, u32, vp, vp, vp, vp, vp, vp]
         L.lk_score_poses.argtypes = [vp, u32, vp, vp, u32] + [vp] * 6
+        L.lk_refine_poses.argtypes = [vp, u32, vp, vp, u32] + [vp] * 5 + [C.c_int] + [vp] * 3
         L.lk_map_stats.argtypes = [vp, vp]
         L.lk_map_slide.argtypes = [vp, vp, vp, vp]
         L.lk_map_memory.argtypes = [vp, vp]
@@ -231,6 +232,30 @@ class Engine:
         self._chk(lib().lk_score_poses(self.h, len(so) - 1, _p(pts), _p(so), n_poses, _p(ps), _p(rot), _p(pos), _p(rot_cov),
                                        _p(pos_cov), _p(out)))
         return out
+
+    def refine_poses(self, pts, set_offsets, pose_set, rot, pos, rot_cov, pos_cov, iters, want_records=True):
+        """lk_refine_poses: every candidate pose refined by `iters` steps of the LiDAR update with P's theta / position
+        blocks held at rot_cov / pos_cov, against the map, touching nothing. Inputs as score_poses. Returns (rot
+        [n_poses, 3, 3], pos [n_poses, 3], records float64 [n_poses, 32] at the refined poses, or None without
+        want_records)."""
+        pts = np.ascontiguousarray(pts, np.float32).reshape(-1, 4)
+        so = np.ascontiguousarray(set_offsets, np.uint32).reshape(-1)
+        if len(so) < 1:
+            raise ValueError("set_offsets needs n_sets + 1 entries")
+        if len(pts) < int(so[-1]):
+            raise ValueError(f"set_offsets ends at point {int(so[-1])}, pts has {len(pts)}")
+        ps = np.ascontiguousarray(pose_set, np.uint32).reshape(-1)
+        n_poses = len(ps)
+        rot = np.ascontiguousarray(rot, np.float64).reshape(n_poses, 9)
+        pos = np.ascontiguousarray(pos, np.float64).reshape(n_poses, 3)
+        rot_cov = np.ascontiguousarray(rot_cov, np.float64).reshape(9)
+        pos_cov = np.ascontiguousarray(pos_cov, np.float64).reshape(9)
+        rot_out, pos_out = np.zeros((n_poses, 3, 3)), np.zeros((n_poses, 3))
+        rec = np.zeros((n_poses, abi.SCORE_STRIDE)) if want_records else None
+        self._chk(lib().lk_refine_poses(self.h, len(so) - 1, _p(pts), _p(so), n_poses, _p(ps), _p(rot), _p(pos),
+                                        _p(rot_cov), _p(pos_cov), int(iters), _p(rot_out), _p(pos_out),
+                                        None if rec is None else _p(rec)))
+        return rot_out, pos_out, rec
 
     def map_slide(self, position):
         """VoxelMapManager::mapSliding (voxel_map.cc:552-571). Returns (slid, removed root voxels)."""
