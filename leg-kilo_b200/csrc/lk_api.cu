@@ -1,5 +1,6 @@
 // lk_api.cu — the extern "C" boundary (include/legkilo_b200.h): context, device memory,
 // staging, launch sequencing. No CPU fallback anywhere: without a CUDA device lk_create fails.
+#include <algorithm>
 #include <climits>
 #include <cmath>
 #include <cstdio>
@@ -13,20 +14,6 @@
 #include "lk_kernels.h"
 #include "lk_mapdev.h"
 
-namespace lk {
-int decode_pointcloud2s_device(uint32_t n_msgs, const uint8_t* const* h_data, const uint32_t* h_n, const double* h_stamps,
-                               const lk_pc2_layout& L, float blind, int filter_num, double time_scale, float* h_pts_out,
-                               float* h_intensity_out, uint32_t* h_out_offs, double* h_begin, double* h_end, DevBuf& scratch,
-                               cudaStream_t s, std::string& err);
-int preprocess_scans_device(uint32_t n_scans, const float* h_pts_in, const uint32_t* h_offs, float leaf, const double* h_begin,
-                            float* h_pts_out, uint32_t* h_scan_off, uint32_t* h_scan_bptr, uint32_t* h_boff, float* h_bcurv,
-                            double* h_btimes, DevBuf& scratch, cudaStream_t s, std::string& err);
-size_t leg_kinematics_scratch_bytes(uint32_t n);
-int leg_kinematics_device(const lk_leg_cfg& cfg, const lk_leg_state* h_in, uint32_t n, int redundancy,
-                          lk_leg_track* track, lk_kinimu_meas* h_out, uint32_t* n_out, void* scratch, cudaStream_t s,
-                          std::string& err);
-}  // namespace lk
-
 using namespace lk;
 
 namespace {
@@ -38,8 +25,6 @@ struct DevView {  // a typed window into somebody else's device allocation
     template <class T>
     T* as() const { return reinterpret_cast<T*>(p); }
 };
-
-constexpr size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
 
 // The packed small inputs of a staged batch (one page-locked block, one H2D copy), byte offsets of
 // chunks | inits | x | P | clk | Q | chunksL | initsL, each 256-byte aligned.
@@ -98,13 +83,7 @@ struct lk_context {
     DevView chunks, stepinit, x_in, P_in, clk_in, Q, x, P, clk, n_eff, status;
     DevBuf dbg_ok, dbg_h, dbg_z, dbg_R, dbg_key, tmp, trace, bar;
     MapInserter inserter;  // UpdateVoxelMap: update_map runs and lk_map_insert
-    // lk_map_insert: one window's points, chunk table + placements (mi_small, staged in h_mi)
-    DevBuf mi_pts, mi_small;
-    PinnedBuf h_mi;
-    // lk_score_poses: points, items | sums | pose constants (staged in h_sp, which also receives the records), the
-    // partial rows of one window, the records
-    DevBuf sp_pts, sp_small, sp_partial, sp_out;
-    PinnedBuf h_sp;
+    PoseScorer scorer;     // lk_score_poses and lk_refine_poses
     int trace_on = 0;
     uint32_t trace_seq = 0;  // fused launches traced since the trace was switched on or last read back
     int lane_cache = 1;
@@ -164,6 +143,8 @@ bool pc2_layout_fits(const lk_pc2_layout& L) {
     return L.lidar_type >= 1 && L.lidar_type <= 3 && L.off_x + 4 <= L.point_step && L.off_y + 4 <= L.point_step &&
            L.off_z + 4 <= L.point_step && L.off_intensity + 4 <= L.point_step && L.off_time + tsz <= L.point_step;
 }
+
+bool all_finite(const double* v, size_t n) { return std::all_of(v, v + n, [](double x) { return std::isfinite(x); }); }
 
 int fail(lk_handle h, int code, const std::string& msg) {
     if (h) h->err = msg;
@@ -920,11 +901,7 @@ static FusedArgs fused_args(lk_handle h, uint32_t first, int iters, bool insert,
         fa.slim_p = h->slim_p && h->n_steps == 1 && !mq && in0.active && in0.t_bucket == ck->last_predict_time &&
                     in0.t_bucket == ck->last_update_time;
     }
-    const MapDev md = h->map.dev();
-    fa.mv.slots = md.slots;
-    fa.mv.hash_mask = md.hash_mask;
-    fa.mv.nodes = md.nodes;
-    fa.mv.hot = md.hot;
+    fa.mv = h->map.view();
     if (mq) {
         fa.imu = mq->d_imu;
         fa.kin = mq->d_kin;
@@ -950,7 +927,7 @@ static FusedArgs fused_args(lk_handle h, uint32_t first, int iters, bool insert,
     fa.g = h->g;
     if (insert) {
         fa.insert = 1;
-        fa.md = md;
+        fa.md = h->map.dev();
         h->inserter.fused_scratch(fa);
     }
     return fa;
@@ -1120,23 +1097,6 @@ static int run_range_impl(lk_handle h, uint32_t first, uint32_t count, int iters
     return rc ? rc : h->inserter.finish(h->map, h->err);
 }
 
-// The ScanConst of a pose given without a filter (lk_map_insert, lk_score_poses), as scan_const_from fills it from one: R, p
-// and the symmetric parts of the theta / position blocks of P (row-major 3 x 3 each).
-static void scan_const_at(const double* R, const double* p, const double* Pt, const double* Pp, ScanConst& sc) {
-    for (int i = 0; i < 9; ++i) sc.R[i] = R[i];
-    for (int i = 0; i < 3; ++i) sc.p[i] = p[i];
-    const int ut[6][2] = {{0, 0}, {0, 1}, {0, 2}, {1, 1}, {1, 2}, {2, 2}};
-    for (int q = 0; q < 6; ++q) {
-        const int i = ut[q][0], j = ut[q][1];
-        sc.Pth[q] = 0.5 * (Pt[i * 3 + j] + Pt[j * 3 + i]);
-        sc.Ppp[q] = 0.5 * (Pp[i * 3 + j] + Pp[j * 3 + i]);
-    }
-}
-
-// lk_map_insert runs its input through the slice-and-sort insert in windows of at most this many points (DESIGN §3.5):
-// per window, the headroom a streaming scan of as many points reserves, and scratch of a fixed size.
-constexpr uint32_t MAP_INSERT_WINDOW = 32768u;
-
 int lk_map_insert(lk_handle h, uint32_t n_sets, const float* pts, const uint32_t* set_offsets, const double* rot,
                   const double* pos, const double* rot_cov, const double* pos_cov) {
     if (!h) return LK_ERR_INVALID_ARG;
@@ -1144,66 +1104,13 @@ int lk_map_insert(lk_handle h, uint32_t n_sets, const float* pts, const uint32_t
     if (!pts || !set_offsets || !rot || !pos || !rot_cov || !pos_cov) return fail(h, LK_ERR_INVALID_ARG, "null argument");
     for (uint32_t s = 0; s < n_sets; ++s) {
         if (set_offsets[s + 1] < set_offsets[s]) return fail(h, LK_ERR_INVALID_ARG, "set_offsets not monotone");
-        bool finite = true;
-        for (int i = 0; i < 9; ++i)
-            finite = finite && std::isfinite(rot[9 * (size_t)s + i]) && std::isfinite(rot_cov[9 * (size_t)s + i]) &&
-                     std::isfinite(pos_cov[9 * (size_t)s + i]);
-        for (int i = 0; i < 3; ++i) finite = finite && std::isfinite(pos[3 * (size_t)s + i]);
-        if (!finite) return fail(h, LK_ERR_INVALID_ARG, "non-finite pose or covariance");
+        if (!all_finite(rot + 9 * (size_t)s, 9) || !all_finite(rot_cov + 9 * (size_t)s, 9) ||
+            !all_finite(pos_cov + 9 * (size_t)s, 9) || !all_finite(pos + 3 * (size_t)s, 3))
+            return fail(h, LK_ERR_INVALID_ARG, "non-finite pose or covariance");
     }
     enter(h);
-    cudaStream_t st = h->stream;
-    const uint32_t W = MAP_INSERT_WINDOW;
-    // a window holds points of at most W sets, and its chunks are 256 points each plus one partial chunk per set
-    const uint32_t max_sets = std::min(n_sets, W);
-    const size_t sc_off = align256(((size_t)W / 256u + max_sets) * sizeof(ChunkDesc));
-    const size_t small_bytes = sc_off + (size_t)max_sets * sizeof(ScanConst);
-    LK_CUDA(h->err, h->mi_pts.ensure((size_t)W * 16));
-    LK_CUDA(h->err, h->mi_small.ensure(small_bytes));
-    LK_CUDA(h->err, h->h_mi.ensure(small_bytes));
-    ChunkDesc* hc = reinterpret_cast<ChunkDesc*>(h->h_mi.p);
-    ScanConst* hs = reinterpret_cast<ScanConst*>((char*)h->h_mi.p + sc_off);
-    const ChunkDesc* dc = reinterpret_cast<const ChunkDesc*>(h->mi_small.p);
-    const ScanConst* ds = reinterpret_cast<const ScanConst*>((char*)h->mi_small.p + sc_off);
-    const uint64_t end = set_offsets[n_sets];
-    uint32_t s = 0;
-    for (uint64_t p0 = set_offsets[0]; p0 < end;) {
-        const uint64_t p1 = std::min<uint64_t>(end, p0 + W);
-        const uint32_t n = (uint32_t)(p1 - p0);
-        int rc = h->inserter.begin(h->map, h->g, n, W, st, h->err);
-        if (rc) return rc;
-        // the window's chunks; ChunkDesc.scan = the set's row in the window's table of placements
-        uint32_t nc = 0, nsc = 0;
-        while (set_offsets[s + 1] <= p0) ++s;
-        for (uint32_t t = s; t < n_sets && set_offsets[t] < p1; ++t) {
-            const uint64_t a = std::max<uint64_t>(set_offsets[t], p0), b = std::min<uint64_t>(set_offsets[t + 1], p1);
-            if (a >= b) continue;
-            scan_const_at(rot + 9 * (size_t)t, pos + 3 * (size_t)t, rot_cov + 9 * (size_t)t, pos_cov + 9 * (size_t)t, hs[nsc]);
-            for (uint64_t q = a; q < b; q += 256) {
-                ChunkDesc& cd = hc[nc++];
-                cd.scan = nsc;
-                cd.start = (uint32_t)(q - p0);
-                cd.count = (uint32_t)std::min<uint64_t>(256, b - q);
-                cd.pad = 0;
-            }
-            ++nsc;
-        }
-        LK_CUDA(h->err, cudaMemcpyAsync(h->mi_pts.p, pts + 4 * p0, (size_t)n * 16, cudaMemcpyHostToDevice, st));
-        // (h_mi is free again: the previous window's sync_counters waited for its copies)
-        LK_CUDA(h->err, cudaMemcpyAsync(h->mi_small.p, hc, (size_t)nc * sizeof(ChunkDesc), cudaMemcpyHostToDevice, st));
-        LK_CUDA(h->err, cudaMemcpyAsync((char*)h->mi_small.p + sc_off, hs, (size_t)nsc * sizeof(ScanConst), cudaMemcpyHostToDevice, st));
-        h->inserter.bucket(h->map, h->g, h->mi_pts.as<float4>(), dc, 0, nc, 0, n, ds, nullptr, st);
-        LK_CUDA(h->err, cudaGetLastError());
-        rc = h->map.sync_counters(st, h->err);
-        if (!rc) rc = h->inserter.finish(h->map, h->err);
-        if (rc) return rc;
-        p0 = p1;
-    }
-    return LK_OK;
+    return h->inserter.insert_sets(h->map, h->g, n_sets, pts, set_offsets, rot, pos, rot_cov, pos_cov, h->stream, h->err);
 }
-
-// lk_score_poses keeps at most this many partial rows (256 bytes each) in flight: poses past it run in the next window.
-constexpr uint32_t SCORE_WINDOW_ROWS = 1u << 18;  // 64 MB
 
 // The inputs lk_score_poses and lk_refine_poses share, checked as the header documents for both (n_poses > 0).
 static int score_check(lk_handle h, uint32_t n_sets, const float* pts, const uint32_t* set_offsets, uint32_t n_poses,
@@ -1213,121 +1120,13 @@ static int score_check(lk_handle h, uint32_t n_sets, const float* pts, const uin
         return fail(h, LK_ERR_INVALID_ARG, "null argument");
     for (uint32_t s = 0; s < n_sets; ++s)
         if (set_offsets[s + 1] < set_offsets[s]) return fail(h, LK_ERR_INVALID_ARG, "set_offsets not monotone");
-    bool finite = true;
-    for (int i = 0; i < 9; ++i) finite = finite && std::isfinite(rot_cov[i]) && std::isfinite(pos_cov[i]);
-    for (uint32_t m = 0; m < n_poses; ++m) {
+    for (uint32_t m = 0; m < n_poses; ++m)
         if (pose_set[m] >= n_sets) return fail(h, LK_ERR_INVALID_ARG, "pose_set names a set past n_sets");
-        for (int i = 0; i < 9; ++i) finite = finite && std::isfinite(rot[9 * (size_t)m + i]);
-        for (int i = 0; i < 3; ++i) finite = finite && std::isfinite(pos[3 * (size_t)m + i]);
-    }
-    if (!finite) return fail(h, LK_ERR_INVALID_ARG, "non-finite pose or covariance");
+    if (!all_finite(rot_cov, 9) || !all_finite(pos_cov, 9) || !all_finite(rot, 9 * (size_t)n_poses) ||
+        !all_finite(pos, 3 * (size_t)n_poses))
+        return fail(h, LK_ERR_INVALID_ARG, "non-finite pose or covariance");
     if (!h->map.ready()) return fail(h, LK_ERR_NOT_READY, "no map: call lk_map_upload or lk_map_build first");
     return LK_OK;
-}
-
-// What score_stage leaves for the launches: the kernels' arguments (one set for every window), the caller's pose index of
-// each pose-table entry, and the item / pose-table start of each window followed by the ends.
-struct ScorePlan {
-    ScoreArgs a;
-    std::vector<uint32_t> ord, win_items, win_sums;
-    size_t out_bytes;  // the records, n_poses * PARTIAL_STRIDE doubles
-};
-
-// The pose table of lk_score_poses / lk_refine_poses in set order (the caller's order within a set), cut into tiles of
-// consecutive poses of one set, and the tiles into windows of at most SCORE_WINDOW_ROWS partial rows (or one tile); item
-// order: tile-major, so the blocks in flight together score one set at neighbouring poses, and touch neighbouring voxels.
-// Sizes the handle's scratch, and queues the points and one packed block (items | sums | ScanConst per pose, pose-table
-// order) on its stream. The staging block h_sp holds at least back_bytes afterwards, for what the caller reads back into it
-// after the H2D copy (same stream).
-static int score_stage(lk_handle h, uint32_t n_sets, const float* pts, const uint32_t* set_offsets, uint32_t n_poses,
-                       const uint32_t* pose_set, const double* rot, const double* pos, const double* rot_cov,
-                       const double* pos_cov, size_t back_bytes, ScorePlan& sp) {
-    cudaStream_t st = h->stream;
-    auto n_chunks = [&](uint32_t s) { return (set_offsets[s + 1] - set_offsets[s] + SCORE_CHUNK - 1) / SCORE_CHUNK; };
-    std::vector<uint32_t> first(n_sets + 1, 0);
-    std::vector<uint32_t>& ord = sp.ord;
-    ord.assign(n_poses, 0);
-    for (uint32_t m = 0; m < n_poses; ++m) ++first[pose_set[m] + 1];
-    for (uint32_t s = 0; s < n_sets; ++s) first[s + 1] += first[s];
-    {
-        std::vector<uint32_t> fill(first.begin(), first.end() - 1);
-        for (uint32_t m = 0; m < n_poses; ++m) ord[fill[pose_set[m]]++] = m;
-    }
-    std::vector<ScoreItem> items;
-    std::vector<ScoreSum> sums(n_poses);
-    std::vector<uint32_t>&win_items = sp.win_items, &win_sums = sp.win_sums;
-    win_items.assign(1, 0);
-    win_sums.assign(1, 0);
-    uint32_t rows = 0;
-    for (uint32_t s = 0; s < n_sets; ++s) {
-        const uint32_t nc = n_chunks(s);
-        const uint32_t tile = std::max<uint32_t>(1, std::min<uint32_t>(SCORE_TILE, nc ? SCORE_WINDOW_ROWS / nc : SCORE_TILE));
-        for (uint32_t p0 = first[s]; p0 < first[s + 1]; p0 += tile) {
-            const uint32_t np = std::min(tile, first[s + 1] - p0);
-            if (rows > 0 && (uint64_t)rows + (uint64_t)np * nc > SCORE_WINDOW_ROWS) {
-                win_items.push_back((uint32_t)items.size());
-                win_sums.push_back(p0);
-                rows = 0;
-            }
-            for (uint32_t c = 0; c < nc; ++c) {
-                ScoreItem it;
-                it.start = set_offsets[s] - set_offsets[0] + c * SCORE_CHUNK;
-                it.count = std::min(SCORE_CHUNK, set_offsets[s + 1] - set_offsets[s] - c * SCORE_CHUNK);
-                it.pose0 = p0;
-                it.n_poses = np;
-                it.row0 = rows + c;
-                it.row_stride = nc;
-                it.pad[0] = it.pad[1] = 0;
-                items.push_back(it);
-            }
-            for (uint32_t k = 0; k < np; ++k) sums[p0 + k] = ScoreSum{rows + k * nc, nc, ord[p0 + k], 0};
-            rows += np * nc;
-        }
-    }
-    win_items.push_back((uint32_t)items.size());
-    win_sums.push_back(n_poses);
-    uint32_t max_rows = 0;
-    for (size_t w = 0; w + 1 < win_sums.size(); ++w)
-        for (uint32_t p = win_sums[w]; p < win_sums[w + 1]; ++p) max_rows = std::max(max_rows, sums[p].row0 + sums[p].n_rows);
-
-    const size_t o_sums = align256(std::max<size_t>(items.size(), 1) * sizeof(ScoreItem));
-    const size_t o_sc = o_sums + align256((size_t)n_poses * sizeof(ScoreSum));
-    const size_t small_bytes = o_sc + (size_t)n_poses * sizeof(ScanConst);
-    sp.out_bytes = (size_t)n_poses * PARTIAL_STRIDE * 8;
-    const uint64_t n_pts = (uint64_t)set_offsets[n_sets] - set_offsets[0];
-    LK_CUDA(h->err, h->sp_pts.ensure(std::max<uint64_t>(n_pts, 1) * 16));
-    LK_CUDA(h->err, h->sp_small.ensure(small_bytes));
-    LK_CUDA(h->err, h->sp_partial.ensure((size_t)std::max<uint32_t>(max_rows, 1) * PARTIAL_STRIDE * 8));
-    LK_CUDA(h->err, h->sp_out.ensure(sp.out_bytes));
-    LK_CUDA(h->err, h->h_sp.ensure(std::max(small_bytes, back_bytes)));
-    char* hb = (char*)h->h_sp.p;
-    std::memcpy(hb, items.data(), items.size() * sizeof(ScoreItem));
-    std::memcpy(hb + o_sums, sums.data(), (size_t)n_poses * sizeof(ScoreSum));
-    ScanConst* hs = reinterpret_cast<ScanConst*>(hb + o_sc);
-    for (uint32_t p = 0; p < n_poses; ++p) scan_const_at(rot + 9 * (size_t)ord[p], pos + 3 * (size_t)ord[p], rot_cov, pos_cov, hs[p]);
-    if (n_pts) LK_CUDA(h->err, cudaMemcpyAsync(h->sp_pts.p, pts + 4 * (size_t)set_offsets[0], n_pts * 16, cudaMemcpyHostToDevice, st));
-    LK_CUDA(h->err, cudaMemcpyAsync(h->sp_small.p, hb, small_bytes, cudaMemcpyHostToDevice, st));
-
-    ScoreArgs& a = sp.a;
-    std::memset(&a, 0, sizeof(a));
-    const MapDev md = h->map.dev();
-    a.pts = h->sp_pts.as<float4>();
-    a.items = h->sp_small.as<ScoreItem>();
-    a.sums = reinterpret_cast<const ScoreSum*>((char*)h->sp_small.p + o_sums);
-    a.sc = reinterpret_cast<const ScanConst*>((char*)h->sp_small.p + o_sc);
-    a.partial = h->sp_partial.as<double>();
-    a.out = h->sp_out.as<double>();
-    a.mv.slots = md.slots; a.mv.hash_mask = md.hash_mask; a.mv.nodes = md.nodes; a.mv.hot = md.hot;
-    a.g = h->g;
-    return LK_OK;
-}
-
-// Window w of a plan: its sums (and k_score_sum's pose-table start) in a, and its item / pose counts.
-static void score_window(ScorePlan& sp, size_t w, uint32_t& n_items, uint32_t& n_sums) {
-    sp.a.item_first = sp.win_items[w];
-    sp.a.sum_first = sp.win_sums[w];
-    n_items = sp.win_items[w + 1] - sp.win_items[w];
-    n_sums = sp.win_sums[w + 1] - sp.win_sums[w];
 }
 
 int lk_score_poses(lk_handle h, uint32_t n_sets, const float* pts, const uint32_t* set_offsets, uint32_t n_poses,
@@ -1338,25 +1137,8 @@ int lk_score_poses(lk_handle h, uint32_t n_sets, const float* pts, const uint32_
     if (!sums_out) return fail(h, LK_ERR_INVALID_ARG, "null argument");
     if (int rc = score_check(h, n_sets, pts, set_offsets, n_poses, pose_set, rot, pos, rot_cov, pos_cov)) return rc;
     enter(h);
-    cudaStream_t st = h->stream;
-    ScorePlan sp;
-    if (int rc = score_stage(h, n_sets, pts, set_offsets, n_poses, pose_set, rot, pos, rot_cov, pos_cov,
-                             (size_t)n_poses * PARTIAL_STRIDE * 8, sp))
-        return rc;
-    // the windows reuse the partial rows in stream order: window w + 1's blocks start after window w's sums are taken
-    for (size_t w = 0; w + 1 < sp.win_items.size(); ++w) {
-        uint32_t n_items, n_sums;
-        score_window(sp, w, n_items, n_sums);
-        launch_score(sp.a, n_items, n_sums, st);
-        LK_CUDA(h->err, cudaGetLastError());
-    }
-    // the one host synchronisation: the staging block is reused for the records only after its H2D copy (same stream)
-    char* hb = (char*)h->h_sp.p;
-    LK_CUDA(h->err, cudaMemcpyAsync(hb, h->sp_out.p, sp.out_bytes, cudaMemcpyDeviceToHost, st));
-    LK_CUDA(h->err, cudaStreamSynchronize(st));
-    LK_CUDA(h->err, cudaGetLastError());
-    std::memcpy(sums_out, hb, sp.out_bytes);
-    return LK_OK;
+    return h->scorer.run(h->map, h->g, n_sets, pts, set_offsets, n_poses, pose_set, rot, pos, rot_cov, pos_cov, 0, nullptr,
+                         nullptr, sums_out, h->stream, h->err);
 }
 
 int lk_refine_poses(lk_handle h, uint32_t n_sets, const float* pts, const uint32_t* set_offsets, uint32_t n_poses,
@@ -1368,40 +1150,8 @@ int lk_refine_poses(lk_handle h, uint32_t n_sets, const float* pts, const uint32
     if (iters < 1) return fail(h, LK_ERR_INVALID_ARG, "iters < 1");
     if (int rc = score_check(h, n_sets, pts, set_offsets, n_poses, pose_set, rot, pos, rot_cov, pos_cov)) return rc;
     enter(h);
-    cudaStream_t st = h->stream;
-    // read back into the staging block: the ScanConst of every pose (pose-table order), then the records if asked for
-    const size_t sc_bytes = (size_t)n_poses * sizeof(ScanConst), o_rec = align256(sc_bytes);
-    ScorePlan sp;
-    if (int rc = score_stage(h, n_sets, pts, set_offsets, n_poses, pose_set, rot, pos, rot_cov, pos_cov,
-                             o_rec + (sums_out ? (size_t)n_poses * PARTIAL_STRIDE * 8 : 0), sp))
-        return rc;
-    // the pose constants the items read are stepped in place: k_score takes them const, k_refine_step writable
-    ScanConst* sc = const_cast<ScanConst*>(sp.a.sc);
-    // window by window, every step of its poses, then (with sums_out) their records at the refined poses; the windows
-    // reuse the partial rows in stream order, and no launch waits for the host
-    for (size_t w = 0; w + 1 < sp.win_items.size(); ++w) {
-        uint32_t n_items, n_sums;
-        score_window(sp, w, n_items, n_sums);
-        for (int it = 0; it < iters; ++it) {
-            launch_score(sp.a, n_items, n_sums, st);
-            launch_refine_step(sp.a, sc, n_sums, st);
-        }
-        if (sums_out) launch_score(sp.a, n_items, n_sums, st);
-        LK_CUDA(h->err, cudaGetLastError());
-    }
-    // the one host synchronisation: the staging block is reused only after its H2D copy (same stream)
-    char* hb = (char*)h->h_sp.p;
-    LK_CUDA(h->err, cudaMemcpyAsync(hb, sc, sc_bytes, cudaMemcpyDeviceToHost, st));
-    if (sums_out) LK_CUDA(h->err, cudaMemcpyAsync(hb + o_rec, h->sp_out.p, sp.out_bytes, cudaMemcpyDeviceToHost, st));
-    LK_CUDA(h->err, cudaStreamSynchronize(st));
-    LK_CUDA(h->err, cudaGetLastError());
-    const ScanConst* hs = reinterpret_cast<const ScanConst*>(hb);
-    for (uint32_t p = 0; p < n_poses; ++p) {
-        std::memcpy(rot_out + 9 * (size_t)sp.ord[p], hs[p].R, sizeof(hs[p].R));
-        std::memcpy(pos_out + 3 * (size_t)sp.ord[p], hs[p].p, sizeof(hs[p].p));
-    }
-    if (sums_out) std::memcpy(sums_out, hb + o_rec, sp.out_bytes);
-    return LK_OK;
+    return h->scorer.run(h->map, h->g, n_sets, pts, set_offsets, n_poses, pose_set, rot, pos, rot_cov, pos_cov, iters, rot_out,
+                         pos_out, sums_out, h->stream, h->err);
 }
 
 int lk_batch_run_range(lk_handle h, uint32_t first, uint32_t count, int iters, int update_map) {

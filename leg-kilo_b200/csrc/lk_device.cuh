@@ -97,6 +97,19 @@ struct ScanConst {
     double Ppp[6];  // sym(P[3:6,3:6]) upper
 };
 
+// The ScanConst of a pose given without a filter (lk_map_insert, lk_score_poses), as scan_const_from fills it from one: R, p
+// and the symmetric parts of the theta / position blocks of P (row-major 3 x 3 each).
+inline void scan_const_at(const double* R, const double* p, const double* Pt, const double* Pp, ScanConst& sc) {
+    for (int i = 0; i < 9; ++i) sc.R[i] = R[i];
+    for (int i = 0; i < 3; ++i) sc.p[i] = p[i];
+    const int ut[6][2] = {{0, 0}, {0, 1}, {0, 2}, {1, 1}, {1, 2}, {2, 2}};
+    for (int q = 0; q < 6; ++q) {
+        const int i = ut[q][0], j = ut[q][1];
+        sc.Pth[q] = 0.5 * (Pt[i * 3 + j] + Pt[j * 3 + i]);
+        sc.Ppp[q] = 0.5 * (Pp[i * 3 + j] + Pp[j * 3 + i]);
+    }
+}
+
 // The block's copy of one scan's constants, one double per thread; the caller synchronises before reading it.
 __device__ __forceinline__ void load_scan_const(ScanConst* dst, const ScanConst* src) {
     const int tid = threadIdx.x;

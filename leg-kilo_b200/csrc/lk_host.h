@@ -1,4 +1,5 @@
-// lk_host.h — host-side owners of device and page-locked memory, and the one CUDA error path of the host code.
+// lk_host.h — host-side owners of device and page-locked memory, the one CUDA error path of the host code, and the host
+// entry points of the units without a launcher in lk_kernels.h.
 // Every cudaMalloc / cudaFree of the library is here: a buffer is freed by its destructor, so no error return leaks.
 #pragma once
 #include <cuda_runtime.h>
@@ -21,6 +22,9 @@
     } while (0)
 
 namespace lk {
+
+// Offsets inside the packed staging blocks are 256-byte aligned.
+constexpr size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
 
 // One device allocation, freed with its owner. Move-only.
 class DevBuf {
@@ -96,5 +100,20 @@ class PinnedBuf {
     void* p = nullptr;
     size_t cap = 0;
 };
+
+// Host entry points of the decode / preprocessing (lk_preprocess.cu) and leg-kinematics (lk_kinematics.cu) units, called
+// behind lk_api.cu's argument checks; each states its preconditions where it is defined. Declared here, which both units
+// include, rather than in lk_kernels.h, whose device headers would give their modules a watchdog note (lk_async.cuh).
+int decode_pointcloud2s_device(uint32_t n_msgs, const uint8_t* const* h_data, const uint32_t* h_n, const double* h_stamps,
+                               const lk_pc2_layout& L, float blind, int filter_num, double time_scale, float* h_pts_out,
+                               float* h_intensity_out, uint32_t* h_out_offs, double* h_begin, double* h_end, DevBuf& scratch,
+                               cudaStream_t s, std::string& err);
+int preprocess_scans_device(uint32_t n_scans, const float* h_pts_in, const uint32_t* h_offs, float leaf, const double* h_begin,
+                            float* h_pts_out, uint32_t* h_scan_off, uint32_t* h_scan_bptr, uint32_t* h_boff, float* h_bcurv,
+                            double* h_btimes, DevBuf& scratch, cudaStream_t s, std::string& err);
+size_t leg_kinematics_scratch_bytes(uint32_t n);
+int leg_kinematics_device(const lk_leg_cfg& cfg, const lk_leg_state* h_in, uint32_t n, int redundancy,
+                          lk_leg_track* track, lk_kinimu_meas* h_out, uint32_t* n_out, void* scratch, cudaStream_t s,
+                          std::string& err);
 
 }  // namespace lk

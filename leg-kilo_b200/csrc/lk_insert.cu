@@ -142,6 +142,10 @@ __global__ void __launch_bounds__(128) k_insert_p4_scan(const __grid_constant__ 
     warp_insert_root_scan(md, a.g, wt, root, a.iroot, a.ipts, a.n_pts, a.pend, lane);
 }
 
+// insert_sets runs its input through the slice-and-sort insert in windows of at most this many points (DESIGN §3.5): per
+// window, the headroom begin reserves for a streaming scan of as many points, and scratch of a fixed size.
+constexpr uint32_t MAP_INSERT_WINDOW = 32768u;
+
 }  // namespace
 
 int MapInserter::begin(MapDevHost& mh, const Globals& g, uint64_t n, uint32_t max_bucket, cudaStream_t s, std::string& err) {
@@ -230,6 +234,58 @@ void MapInserter::fused_scratch(FusedArgs& fa) const {
     fa.pend = pend_.as<int>();
     fa.touched = touched_.as<uint32_t>();
     fa.ins_counters = counters_.as<uint32_t>() + 2;
+}
+
+int MapInserter::insert_sets(MapDevHost& mh, const Globals& g, uint32_t n_sets, const float* pts, const uint32_t* set_offsets,
+                             const double* rot, const double* pos, const double* rot_cov, const double* pos_cov,
+                             cudaStream_t st, std::string& err) {
+    const uint32_t W = MAP_INSERT_WINDOW;
+    // a window holds points of at most W sets, and its chunks are 256 points each plus one partial chunk per set
+    const uint32_t max_sets = std::min(n_sets, W);
+    const size_t sc_off = align256(((size_t)W / 256u + max_sets) * sizeof(ChunkDesc));
+    const size_t small_bytes = sc_off + (size_t)max_sets * sizeof(ScanConst);
+    LK_CUDA(err, win_pts_.ensure((size_t)W * 16));
+    LK_CUDA(err, win_small_.ensure(small_bytes));
+    LK_CUDA(err, h_win_.ensure(small_bytes));
+    ChunkDesc* hc = reinterpret_cast<ChunkDesc*>(h_win_.p);
+    ScanConst* hs = reinterpret_cast<ScanConst*>((char*)h_win_.p + sc_off);
+    const ChunkDesc* dc = reinterpret_cast<const ChunkDesc*>(win_small_.p);
+    const ScanConst* ds = reinterpret_cast<const ScanConst*>((char*)win_small_.p + sc_off);
+    const uint64_t end = set_offsets[n_sets];
+    uint32_t s = 0;
+    for (uint64_t p0 = set_offsets[0]; p0 < end;) {
+        const uint64_t p1 = std::min<uint64_t>(end, p0 + W);
+        const uint32_t n = (uint32_t)(p1 - p0);
+        int rc = begin(mh, g, n, W, st, err);
+        if (rc) return rc;
+        // the window's chunks; ChunkDesc.scan = the set's row in the window's table of placements
+        uint32_t nc = 0, nsc = 0;
+        while (set_offsets[s + 1] <= p0) ++s;
+        for (uint32_t t = s; t < n_sets && set_offsets[t] < p1; ++t) {
+            const uint64_t a = std::max<uint64_t>(set_offsets[t], p0), b = std::min<uint64_t>(set_offsets[t + 1], p1);
+            if (a >= b) continue;
+            scan_const_at(rot + 9 * (size_t)t, pos + 3 * (size_t)t, rot_cov + 9 * (size_t)t, pos_cov + 9 * (size_t)t, hs[nsc]);
+            for (uint64_t q = a; q < b; q += 256) {
+                ChunkDesc& cd = hc[nc++];
+                cd.scan = nsc;
+                cd.start = (uint32_t)(q - p0);
+                cd.count = (uint32_t)std::min<uint64_t>(256, b - q);
+                cd.pad = 0;
+            }
+            ++nsc;
+        }
+        LK_CUDA(err, cudaMemcpyAsync(win_pts_.p, pts + 4 * p0, (size_t)n * 16, cudaMemcpyHostToDevice, st));
+        // (h_win_ is free again: the previous window's sync_counters waited for its copies)
+        LK_CUDA(err, cudaMemcpyAsync(win_small_.p, hc, (size_t)nc * sizeof(ChunkDesc), cudaMemcpyHostToDevice, st));
+        LK_CUDA(err, cudaMemcpyAsync((char*)win_small_.p + sc_off, hs, (size_t)nsc * sizeof(ScanConst), cudaMemcpyHostToDevice, st));
+        bucket(mh, g, win_pts_.as<float4>(), dc, 0, nc, 0, n, ds, nullptr, st);
+        LK_CUDA(err, cudaGetLastError());
+        rc = mh.sync_counters(st, err);
+        if (!rc) rc = finish(mh, err);
+        if (rc) return rc;
+        p0 = p1;
+    }
+    return LK_OK;
 }
 
 }  // namespace lk

@@ -103,35 +103,6 @@ void launch_filter_obs(double* x, double* P, const double* Q, lk_stream_clock* c
 void launch_update_by_points(double* x, double* P, uint32_t n, const double* h, const double* z, const double* r,
                              cudaStream_t s);
 
-// ---- lk_score_poses (lk_score.cu) ---------------------------------------------------------------
-constexpr uint32_t SCORE_CHUNK = 256;  // points per block: one per thread
-constexpr uint32_t SCORE_TILE = 16;    // poses per block
-// One block of k_score: points [start, start + count) of one set against poses [pose0, pose0 + n_poses) of the pose table
-// (consecutive poses of that set); pose pose0 + k writes partial row row0 + k * row_stride.
-struct ScoreItem {
-    uint32_t start, count, pose0, n_poses, row0, row_stride, pad[2];
-};
-// One block of k_score_sum: partial rows [row0, row0 + n_rows) summed into record `pose` of out.
-struct ScoreSum {
-    uint32_t row0, n_rows, pose, pad;
-};
-struct ScoreArgs {
-    const float4* pts;
-    const ScoreItem* items;
-    uint32_t item_first;  // first item of this launch (grid.x = number of items)
-    const ScoreSum* sums;
-    uint32_t sum_first;
-    const ScanConst* sc;  // one per pose, in the order the items address them
-    double* partial;      // [rows of the window * PARTIAL_STRIDE]
-    double* out;          // [n_poses * PARTIAL_STRIDE], by the caller's pose index
-    MapView mv;
-    Globals g;
-};
-void launch_score(const ScoreArgs& a, uint32_t n_items, uint32_t n_sums, cudaStream_t s);
-// lk_refine_poses: one pose step (k_refine_step) for poses [sum_first, sum_first + n_sums) of the pose table, from the
-// records a.out holds at their current poses; the new R / p are written into sc, the same buffer as a.sc.
-void launch_refine_step(const ScoreArgs& a, ScanConst* sc, uint32_t n_sums, cudaStream_t s);
-
 // ---- fused per-scan persistent kernel (lk_fused.cu) -------------------------------------------
 constexpr int FUSED_INLINE_STEPS = 64;
 // Small inputs carried in the kernel's parameter block (direct mode: no staging copy before the launch).

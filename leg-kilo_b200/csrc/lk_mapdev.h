@@ -23,6 +23,7 @@ class MapDevHost {
                         std::string& err);
     void release();  // drop the map (the reserve and the tile size stay)
     MapDev dev() const;
+    MapView view() const;  // what the residual path reads of dev()
     bool ready() const { return hash_cap != 0; }
     // pull the device allocator counters (free lists included) into the host mirrors
     int sync_counters(cudaStream_t s, std::string& err);
@@ -80,11 +81,39 @@ class MapInserter {
     // Once the stream is synchronised after the launches: report pools that ran out (push_counters clears the flag).
     int finish(const MapDevHost& mh, std::string& err) const;
     void fused_scratch(FusedArgs& fa) const;  // the scratch k_scan_fused<…, INS> inserts through
+    // lk_map_insert behind its argument checks (n_sets >= 1): set t is float4 points [set_offsets[t], set_offsets[t + 1]) of
+    // pts placed at (rot, pos) with the theta / position blocks (rot_cov, pos_cov), row-major 3 x 3 each. Runs in windows of
+    // at most MAP_INSERT_WINDOW points, each one bucket between begin and finish, so the stream is synchronised per window.
+    int insert_sets(MapDevHost& mh, const Globals& g, uint32_t n_sets, const float* pts, const uint32_t* set_offsets,
+                    const double* rot, const double* pos, const double* rot_cov, const double* pos_cov, cudaStream_t s,
+                    std::string& err);
 
    private:
     DevBuf pts_, root_, touched_, list_, counters_, pend_;  // InsertArgs; counters: [2..3] are the two-launch path's
     uint64_t pend_nodes_ = 0;  // nodes pend_ covers
     uint32_t parity_ = 0;      // the two-launch counter of the next small bucket
+    // insert_sets: one window's points, its chunk table + placements (win_small_, staged in h_win_)
+    DevBuf win_pts_, win_small_;
+    PinnedBuf h_win_;
+};
+// lk_score.cu — lk_score_poses and lk_refine_poses (DESIGN §3.11, §3.12), one per handle. Its scratch is stream-ordered; no
+// call keeps its contents.
+class PoseScorer {
+   public:
+    // Behind the calls' argument checks (n_poses >= 1, a map): the records of every pose of pose_set (rot / pos per pose,
+    // one rot_cov / pos_cov for all), after iters refinement steps of each pose (0 = score only). Reads back the poses into
+    // rot_out / pos_out and the records at them into sums_out, each when not null, in the caller's pose order. One host
+    // synchronisation.
+    int run(const MapDevHost& mh, const Globals& g, uint32_t n_sets, const float* pts, const uint32_t* set_offsets,
+            uint32_t n_poses, const uint32_t* pose_set, const double* rot, const double* pos, const double* rot_cov,
+            const double* pos_cov, int iters, double* rot_out, double* pos_out, double* sums_out, cudaStream_t s,
+            std::string& err);
+
+   private:
+    // points, items | sums | ScanConst per pose (staged in h_, which also receives the read-back), the partial rows of one
+    // window, the records
+    DevBuf pts_, small_, partial_, out_;
+    PinnedBuf h_;
 };
 // lk_mapio.cu
 int map_upload_blob(MapDevHost& mh, const Globals& g, const void* blob, size_t bytes, cudaStream_t s, std::string& err);

@@ -167,6 +167,11 @@ MapDev MapDevHost::dev() const {
     return d;
 }
 
+MapView MapDevHost::view() const {
+    const MapDev d = dev();
+    return {d.slots, d.hash_mask, d.nodes, d.hot};
+}
+
 int MapDevHost::allocate(uint64_t roots, uint64_t nnodes, uint64_t npoints, cudaStream_t s, std::string& err) {
     // Pools that are large enough are kept; a pool that is not is freed before its replacement is allocated. Any
     // failure drops the whole map, so no caller goes ahead on a half-built one.

@@ -16,7 +16,15 @@
 // k_refine_step (lk_refine_poses): one warp per pose, one pose step from the pose's record: the information-form solve of
 // block_solve_state (its column assembly, warp_solve6) with the pose's P66 held, and State::operator+= on R and p, written into
 // the pose's ScanConst in place. Steps chain on the device: k_score, k_score_sum, k_refine_step, k_score, ...
+//
+// PoseScorer (lk_mapdev.h) is the host plan both calls run: the pose table, its tiles and windows, one packed H2D copy, the
+// launches of every window, one read-back and one host synchronisation.
+#include <algorithm>
+#include <cstring>
+#include <vector>
+
 #include "lk_kernels.h"
+#include "lk_mapdev.h"
 #include "lk_pass.cuh"
 #include "lk_solve.cuh"
 
@@ -25,6 +33,32 @@ namespace lk {
 static_assert(LK_SCORE_A == 0 && LK_SCORE_B == ACC_B && LK_SCORE_SUM_R == ACC_SUMR && LK_SCORE_COUNT == ACC_CNT &&
                   LK_SCORE_SUM_Z2R == NACC && LK_SCORE_STRIDE == PARTIAL_STRIDE,
               "lk_score_poses record layout (include/legkilo_b200.h) = the partial-row layout");
+
+constexpr uint32_t SCORE_CHUNK = 256;  // points per block: one per thread
+constexpr uint32_t SCORE_TILE = 16;    // poses per block
+// A call keeps at most this many partial rows (256 bytes each) in flight: poses past it run in the next window.
+constexpr uint32_t SCORE_WINDOW_ROWS = 1u << 18;  // 64 MB
+// One block of k_score: points [start, start + count) of one set against poses [pose0, pose0 + n_poses) of the pose table
+// (consecutive poses of that set); pose pose0 + k writes partial row row0 + k * row_stride.
+struct ScoreItem {
+    uint32_t start, count, pose0, n_poses, row0, row_stride, pad[2];
+};
+// One block of k_score_sum: partial rows [row0, row0 + n_rows) summed into record `pose` of out.
+struct ScoreSum {
+    uint32_t row0, n_rows, pose, pad;
+};
+struct ScoreArgs {
+    const float4* pts;
+    const ScoreItem* items;
+    uint32_t item_first;  // first item of this launch (grid.x = number of items)
+    const ScoreSum* sums;
+    uint32_t sum_first;
+    const ScanConst* sc;  // one per pose, in the order the items address them
+    double* partial;      // [rows of the window * PARTIAL_STRIDE]
+    double* out;          // [n_poses * PARTIAL_STRIDE], by the caller's pose index
+    MapView mv;
+    Globals g;
+};
 
 namespace {
 
@@ -146,9 +180,124 @@ void launch_score(const ScoreArgs& a, uint32_t n_items, uint32_t n_sums, cudaStr
     if (n_sums) k_score_sum<<<n_sums, SUM_THREADS, 0, s>>>(a);
 }
 
+// One pose step (k_refine_step) for poses [sum_first, sum_first + n_sums) of the pose table, from the records a.out holds
+// at their current poses; the new R / p are written into sc, the same buffer as a.sc.
 void launch_refine_step(const ScoreArgs& a, ScanConst* sc, uint32_t n_sums, cudaStream_t s) {
     constexpr uint32_t per_block = REFINE_THREADS / 32;
     if (n_sums) k_refine_step<<<(n_sums + per_block - 1) / per_block, REFINE_THREADS, 0, s>>>(a, sc, n_sums);
+}
+
+int PoseScorer::run(const MapDevHost& mh, const Globals& g, uint32_t n_sets, const float* pts, const uint32_t* set_offsets,
+                    uint32_t n_poses, const uint32_t* pose_set, const double* rot, const double* pos, const double* rot_cov,
+                    const double* pos_cov, int iters, double* rot_out, double* pos_out, double* sums_out, cudaStream_t st,
+                    std::string& err) {
+    // The pose table in set order (ord: the caller's pose index of each entry, the caller's order within a set), cut into
+    // tiles of consecutive poses of one set, and the tiles into windows of at most SCORE_WINDOW_ROWS partial rows (or one
+    // tile); window w is items [win_items[w], win_items[w + 1]) and pose-table entries [win_sums[w], win_sums[w + 1]). Item
+    // order: tile-major, so the blocks in flight together score one set at neighbouring poses, and touch neighbouring voxels.
+    auto n_chunks = [&](uint32_t s) { return (set_offsets[s + 1] - set_offsets[s] + SCORE_CHUNK - 1) / SCORE_CHUNK; };
+    std::vector<uint32_t> first(n_sets + 1, 0), ord(n_poses, 0);
+    for (uint32_t m = 0; m < n_poses; ++m) ++first[pose_set[m] + 1];
+    for (uint32_t s = 0; s < n_sets; ++s) first[s + 1] += first[s];
+    {
+        std::vector<uint32_t> fill(first.begin(), first.end() - 1);
+        for (uint32_t m = 0; m < n_poses; ++m) ord[fill[pose_set[m]]++] = m;
+    }
+    std::vector<ScoreItem> items;
+    std::vector<ScoreSum> sums(n_poses);
+    std::vector<uint32_t> win_items(1, 0), win_sums(1, 0);
+    uint32_t rows = 0;
+    for (uint32_t s = 0; s < n_sets; ++s) {
+        const uint32_t nc = n_chunks(s);
+        const uint32_t tile = std::max<uint32_t>(1, std::min<uint32_t>(SCORE_TILE, nc ? SCORE_WINDOW_ROWS / nc : SCORE_TILE));
+        for (uint32_t p0 = first[s]; p0 < first[s + 1]; p0 += tile) {
+            const uint32_t np = std::min(tile, first[s + 1] - p0);
+            if (rows > 0 && (uint64_t)rows + (uint64_t)np * nc > SCORE_WINDOW_ROWS) {
+                win_items.push_back((uint32_t)items.size());
+                win_sums.push_back(p0);
+                rows = 0;
+            }
+            for (uint32_t c = 0; c < nc; ++c) {
+                ScoreItem it;
+                it.start = set_offsets[s] - set_offsets[0] + c * SCORE_CHUNK;
+                it.count = std::min(SCORE_CHUNK, set_offsets[s + 1] - set_offsets[s] - c * SCORE_CHUNK);
+                it.pose0 = p0;
+                it.n_poses = np;
+                it.row0 = rows + c;
+                it.row_stride = nc;
+                it.pad[0] = it.pad[1] = 0;
+                items.push_back(it);
+            }
+            for (uint32_t k = 0; k < np; ++k) sums[p0 + k] = ScoreSum{rows + k * nc, nc, ord[p0 + k], 0};
+            rows += np * nc;
+        }
+    }
+    win_items.push_back((uint32_t)items.size());
+    win_sums.push_back(n_poses);
+    uint32_t max_rows = 0;
+    for (size_t w = 0; w + 1 < win_sums.size(); ++w)
+        for (uint32_t p = win_sums[w]; p < win_sums[w + 1]; ++p) max_rows = std::max(max_rows, sums[p].row0 + sums[p].n_rows);
+
+    // One packed block, items | sums | ScanConst per pose (pose-table order), and one H2D copy. The staging block h_ then
+    // receives the read-back: the ScanConst of every pose if rot_out is set, then the records if sums_out is.
+    const size_t o_sums = align256(std::max<size_t>(items.size(), 1) * sizeof(ScoreItem));
+    const size_t o_sc = o_sums + align256((size_t)n_poses * sizeof(ScoreSum));
+    const size_t sc_bytes = (size_t)n_poses * sizeof(ScanConst), small_bytes = o_sc + sc_bytes;
+    const size_t out_bytes = (size_t)n_poses * PARTIAL_STRIDE * 8;
+    const size_t o_rec = rot_out ? align256(sc_bytes) : 0, back_bytes = o_rec + (sums_out ? out_bytes : 0);
+    const uint64_t n_pts = (uint64_t)set_offsets[n_sets] - set_offsets[0];
+    LK_CUDA(err, pts_.ensure(std::max<uint64_t>(n_pts, 1) * 16));
+    LK_CUDA(err, small_.ensure(small_bytes));
+    LK_CUDA(err, partial_.ensure((size_t)std::max<uint32_t>(max_rows, 1) * PARTIAL_STRIDE * 8));
+    LK_CUDA(err, out_.ensure(out_bytes));
+    LK_CUDA(err, h_.ensure(std::max(small_bytes, back_bytes)));
+    char* hb = (char*)h_.p;
+    std::memcpy(hb, items.data(), items.size() * sizeof(ScoreItem));
+    std::memcpy(hb + o_sums, sums.data(), (size_t)n_poses * sizeof(ScoreSum));
+    ScanConst* hs = reinterpret_cast<ScanConst*>(hb + o_sc);
+    for (uint32_t p = 0; p < n_poses; ++p) scan_const_at(rot + 9 * (size_t)ord[p], pos + 3 * (size_t)ord[p], rot_cov, pos_cov, hs[p]);
+    if (n_pts) LK_CUDA(err, cudaMemcpyAsync(pts_.p, pts + 4 * (size_t)set_offsets[0], n_pts * 16, cudaMemcpyHostToDevice, st));
+    LK_CUDA(err, cudaMemcpyAsync(small_.p, hb, small_bytes, cudaMemcpyHostToDevice, st));
+
+    // the pose constants the items read are stepped in place: k_score takes them const, k_refine_step writable
+    ScanConst* sc = reinterpret_cast<ScanConst*>((char*)small_.p + o_sc);
+    ScoreArgs a;
+    std::memset(&a, 0, sizeof(a));
+    a.pts = pts_.as<float4>();
+    a.items = small_.as<ScoreItem>();
+    a.sums = reinterpret_cast<const ScoreSum*>((char*)small_.p + o_sums);
+    a.sc = sc;
+    a.partial = partial_.as<double>();
+    a.out = out_.as<double>();
+    a.mv = mh.view();
+    a.g = g;
+    // window by window, every step of its poses, then (with sums_out) their records at the final poses; the windows reuse
+    // the partial rows in stream order, and no launch waits for the host
+    for (size_t w = 0; w + 1 < win_items.size(); ++w) {
+        a.item_first = win_items[w];
+        a.sum_first = win_sums[w];
+        const uint32_t n_items = win_items[w + 1] - win_items[w], n_sums = win_sums[w + 1] - win_sums[w];
+        for (int it = 0; it < iters; ++it) {
+            launch_score(a, n_items, n_sums, st);
+            launch_refine_step(a, sc, n_sums, st);
+        }
+        if (sums_out) launch_score(a, n_items, n_sums, st);
+        LK_CUDA(err, cudaGetLastError());
+    }
+    // the one host synchronisation: the staging block is reused only after its H2D copy (same stream)
+    if (rot_out) LK_CUDA(err, cudaMemcpyAsync(hb, sc, sc_bytes, cudaMemcpyDeviceToHost, st));
+    if (sums_out) LK_CUDA(err, cudaMemcpyAsync(hb + o_rec, out_.p, out_bytes, cudaMemcpyDeviceToHost, st));
+    LK_CUDA(err, cudaStreamSynchronize(st));
+    LK_CUDA(err, cudaGetLastError());
+    if (rot_out) {
+        const ScanConst* hr = reinterpret_cast<const ScanConst*>(hb);
+        for (uint32_t p = 0; p < n_poses; ++p) {
+            std::memcpy(rot_out + 9 * (size_t)ord[p], hr[p].R, sizeof(hr[p].R));
+            std::memcpy(pos_out + 3 * (size_t)ord[p], hr[p].p, sizeof(hr[p].p));
+        }
+    }
+    if (sums_out) std::memcpy(sums_out, hb + o_rec, out_bytes);
+    return LK_OK;
 }
 
 }  // namespace lk

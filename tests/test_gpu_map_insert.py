@@ -27,7 +27,7 @@ from legkilo_b200 import Engine, LkError, abi, lib, synth
 from test_map_insert_oracle import fixture
 
 pytestmark = pytest.mark.gpu
-WINDOW = 32768  # lk_api.cu: MAP_INSERT_WINDOW
+WINDOW = 32768  # lk_insert.cu: MAP_INSERT_WINDOW
 
 
 def exact(a, b):

@@ -23,7 +23,7 @@ for p in ("leg-kilo_b200/python", "oracle"):
 import lko_insert  # noqa: E402
 from legkilo_b200 import Engine, abi, synth  # noqa: E402
 
-WINDOW = 32768  # lk_api.cu: MAP_INSERT_WINDOW
+WINDOW = 32768  # lk_insert.cu: MAP_INSERT_WINDOW
 
 
 def trajectory(cfg, n_scans):
