@@ -275,6 +275,16 @@ __device__ __noinline__ void fused_finish(SM* sm, const FusedArgs& a, const Step
     FT(22);
 }
 
+// The all-reduce's shared-memory scratch (ll_allreduce: LL_XS doubles) lives in the pass's point contexts: a pass writes
+// every context it reads (points_pass) and ends with a block barrier, and the exchange ends with one before the next pass,
+// so the two never overlap. Between buckets the contexts are dead too (the predict scratch and the insert use other
+// memory), which covers the barriers of grid_sync.
+template <class SM>
+__device__ __forceinline__ double* ll_scratch(SM* sm) { return reinterpret_cast<double*>(sm->u.pass.pt); }
+static_assert(sizeof(PassHot::pt) >= LL_XS * sizeof(double) && sizeof(PassNodes::pt) >= LL_XS * sizeof(double) &&
+                  alignof(PointCtx) >= alignof(double),
+              "the all-reduce's scratch must fit in the point contexts");
+
 template <bool INL> struct InlineSel { typedef FusedInline type; };
 template <> struct InlineSel<false> { typedef FusedNoInline type; };
 
@@ -284,10 +294,11 @@ template <> struct InlineSel<false> { typedef FusedNoInline type; };
 // a line cached before another SM rewrote it; the read-only path (ld.global.nc) is not used on the map in these kernels.
 // The next bucket's pass reads the node records the insert just wrote with generic stores through bulk copies (async
 // proxy): a proxy fence after the acquire orders the two.
-__device__ __forceinline__ void grid_sync(const FusedArgs& a, uint32_t& sync_idx) {
+template <class SM>
+__device__ __forceinline__ void grid_sync(SM* sm, const FusedArgs& a, uint32_t& sync_idx) {
     __threadfence();
     __syncthreads();
-    if (threadIdx.x < 32) (void)ll_allreduce(a.ll, sync_idx & 1u, a.epoch + sync_idx, blockIdx.x, gridDim.x, 0.0, (int)threadIdx.x);
+    (void)ll_allreduce<WARPS>(a.ll, sync_idx & 1u, a.epoch + sync_idx, blockIdx.x, gridDim.x, 0.0, ll_scratch(sm));
     ++sync_idx;
     __syncthreads();
     __threadfence();
@@ -410,9 +421,9 @@ __global__ void __launch_bounds__(BLOCK, 1) k_scan_fused(const __grid_constant__
                 FT(31);
                 return;
             }
-            // 2) all-reduce of the block rows (warp 0), no barrier
+            // 2) all-reduce of the block rows, no grid barrier: warp 0 stores, every warp polls
+            double v = 0.0;
             if (warp == 0) {
-                double v = 0.0;
 #pragma unroll
                 for (int w = 0; w < WARPS; ++w) v += sm->slice[w * 32 + lane];
                 if (!dep_waited) {  // the rows / outputs of the previous launch
@@ -420,9 +431,10 @@ __global__ void __launch_bounds__(BLOCK, 1) k_scan_fused(const __grid_constant__
                     asm volatile("griddepcontrol.wait;" ::: "memory");
                     FT(24);
                 }
-                sm->f.acc[lane] = ll_allreduce(a.ll, it_global & 1u, a.epoch + it_global, blockIdx.x, n_chunks, v, lane, FT_HOPS(),
-                                               a.finishers, it_global >= 2);
             }
+            const double t = ll_allreduce<WARPS>(a.ll, it_global & 1u, a.epoch + it_global, blockIdx.x, n_chunks, v, ll_scratch(sm),
+                                                 FT_HOPS(), a.finishers, it_global >= 2);
+            if (warp == 0) sm->f.acc[lane] = t;
             dep_waited = true;
             __syncthreads();
             FTI(3 + it_global * 4);
@@ -467,7 +479,7 @@ __global__ void __launch_bounds__(BLOCK, 1) k_scan_fused(const __grid_constant__
                 a.world[my_start + tid] = o;
                 a.iroot[li] = insert_register_point(md, a.g, p, a.pend, a.touched, &a.ins_counters[cslot]);
             }
-            grid_sync(a, it_global);
+            grid_sync(sm, a, it_global);
             FTS(6);
             // Phase 2, every warp of every block: one touched root at a time, its points in index order
             {
@@ -476,7 +488,7 @@ __global__ void __launch_bounds__(BLOCK, 1) k_scan_fused(const __grid_constant__
                 fused_insert_phase2(reinterpret_cast<FusedSmemIns*>(smem_raw), a.touched, a.iroot, a.ipts, a.pend, n_touched, n_bucket);
                 cslot ^= 1u;
             }
-            grid_sync(a, it_global);
+            grid_sync(sm, a, it_global);
             FTS(7);
         }
     }
