@@ -209,7 +209,9 @@ int lk_host_free(void* p);
 int lk_set_param(lk_handle h, const char* name, double value);
 
 /* Debug read-back (what: 0 = per-chunk partial sums, 1 = scan constants, 2 = %globaltimer trace,
- * 3 = host-side phase times of lk_scan_update [stage, enqueue, wait+fetch, calls] in ns (reading resets)). */
+ * 3 = host-side phase times of lk_scan_update [stage, enqueue, wait+fetch, calls] in ns (reading resets),
+ * 4 = the scratch the pose scorer holds (lk_score_poses, lk_refine_poses, lk_search_poses): two uint64, device bytes and
+ * page-locked bytes). */
 int lk_debug_read(lk_handle h, int what, void* dst, size_t bytes);
 
 /* ---- map ------------------------------------------------------------------------------- */
@@ -322,6 +324,43 @@ int lk_score_poses(lk_handle h, uint32_t n_sets, const float* pts, const uint32_
 int lk_refine_poses(lk_handle h, uint32_t n_sets, const float* pts, const uint32_t* set_offsets, uint32_t n_poses,
                     const uint32_t* pose_set, const double* rot, const double* pos, const double* rot_cov,
                     const double* pos_cov, int iters, double* rot_out, double* pos_out, double* sums_out);
+/* The search of INTEGRATION.md §5 in one call: a lattice of candidate poses per point set, scored, the best k kept, refined
+ * and re-scored, with nothing per candidate leaving the device. No filter, map or staged batch is touched.
+ * Set s = pts[set_offsets[s] .. set_offsets[s+1]), as in lk_score_poses. Its candidates are its attitudes
+ * att_offsets[s] .. att_offsets[s+1] (row-major 3x3 each in att_rot, body->world) times one position lattice of
+ * counts = (nx, ny, nz) points spaced step, anchored at origin[3s..]. With L = nx ny nz, candidate c of set s is
+ *   a = c / L, r = c % L, ix = r % nx, iy = (r / nx) % ny, iz = r / (nx ny),
+ *   rot = att_rot[9 (att_offsets[s] + a) ..],  pos[j] = origin[3s + j] + (double)i_j * step[j]
+ * (the product rounded to double, then the sum: no fused multiply-add).
+ * The result is, bitwise, this composition of the other calls, per set s:
+ *   1. every candidate of s scored as lk_score_poses scores it, with rot_cov / pos_cov;
+ *   2. the k best kept, ordered by (count descending, candidate index ascending), a total order;
+ *   3. those refined as lk_refine_poses(iters) refines them, with rot_cov / pos_cov;
+ *   4. the refined poses scored as lk_score_poses scores them, with rot_cov_tight / pos_cov_tight;
+ *   5. ordered by (tight count descending, rank in step 2 ascending).
+ * Entry s k + j of each output is the j-th of step 5: rot_out 9 doubles, pos_out 3, sums_out LK_SCORE_STRIDE (the tight
+ * record, LK_SCORE_*), cand_out 1 (its candidate index c). A set's outputs depend only on that set, its candidates, the
+ * four blocks, iters and k: not on the other sets, their order or how the call is cut into windows.
+ * LK_ERR_NOT_READY: the handle has no map. LK_ERR_INVALID_ARG: a NULL argument with n_sets > 0, set_offsets or att_offsets
+ * not monotone, a zero entry of counts, k of 0 or above LK_SEARCH_MAX_K, iters < 1, a non-finite entry of the attitudes,
+ * origin, step or any block, or a set with fewer than k candidates or with 2^32 or more. On any error nothing is written.
+ * n_sets == 0 does nothing.
+ * Runs on the device with one host synchronisation, whatever the number of candidates: they are generated, scored and
+ * kept window by window on the device (windows of at most 262 144 candidates and 262 144 partial rows). Device memory,
+ * shared with lk_score_poses and lk_refine_poses, kept by the handle and grown to the largest call, does not depend on the
+ * number of candidates: at most 16 bytes per point, 72 bytes per set and per attitude, 1 024 bytes per kept pose
+ * (n_sets k) plus 32 bytes per (256-point chunk of a set, tile of up to 16 of its kept poses), and 192 MiB for one window
+ * (64 MiB of partial rows, 64 MiB of records, 64 MiB for the window's 192-byte pose constants, sums and items), each buffer
+ * with up to 1/8 growth slack. Page-locked staging: the larger of (72 bytes per set and per attitude, 16 bytes per kept
+ * pose and 32 per (chunk, tile) of them) and 356 bytes per kept pose, plus alignment and 1/4 growth slack.
+ * lk_debug_read(h, 4, ...) reads back what is held. */
+#define LK_SEARCH_MAX_K 256
+int lk_search_poses(lk_handle h, uint32_t n_sets, const float* pts, const uint32_t* set_offsets,
+                    const uint32_t* att_offsets, const double* att_rot, const double* origin,
+                    const double step[3], const uint32_t counts[3],
+                    const double* rot_cov, const double* pos_cov, int iters,
+                    const double* rot_cov_tight, const double* pos_cov_tight, uint32_t k,
+                    double* rot_out, double* pos_out, double* sums_out, uint32_t* cand_out);
 /* Map counters: out[0]=roots, out[1]=nodes, out[2]=retained points, out[3]=plane nodes. */
 int lk_map_stats(lk_handle h, uint64_t out[4]);
 /* VoxelMapManager::mapSliding + clearMemOutOfMap (voxel_map.cc:552-594; dead code in the reference, needed for unbounded

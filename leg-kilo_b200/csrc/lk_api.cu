@@ -459,12 +459,17 @@ int lk_set_param(lk_handle h, const char* name, double value) {
     return fail(h, LK_ERR_INVALID_ARG, std::string("unknown parameter ") + name);
 }
 
-// Debug read-back of internal device buffers: what = 0 partial sums, 1 scan constants.
+// Debug read-back of internal device buffers: what = 0 partial sums, 1 scan constants (the header lists the rest).
 int lk_debug_read(lk_handle h, int what, void* dst, size_t bytes) {
     if (!h || !dst) return LK_ERR_INVALID_ARG;
     if (what == 3) {  // host-side phase times of lk_scan_update (ns, accumulated) — reading resets them
         std::memcpy(dst, h->hprof, std::min(bytes, sizeof(h->hprof)));
         std::memset(h->hprof, 0, sizeof(h->hprof));
+        return LK_OK;
+    }
+    if (what == 4) {  // the pose scorer's scratch: device bytes, page-locked bytes
+        const uint64_t held[2] = {h->scorer.device_bytes(), h->scorer.host_bytes()};
+        std::memcpy(dst, held, std::min(bytes, sizeof(held)));
         return LK_OK;
     }
     enter(h);
@@ -1152,6 +1157,40 @@ int lk_refine_poses(lk_handle h, uint32_t n_sets, const float* pts, const uint32
     enter(h);
     return h->scorer.run(h->map, h->g, n_sets, pts, set_offsets, n_poses, pose_set, rot, pos, rot_cov, pos_cov, iters, rot_out,
                          pos_out, sums_out, h->stream, h->err);
+}
+
+int lk_search_poses(lk_handle h, uint32_t n_sets, const float* pts, const uint32_t* set_offsets, const uint32_t* att_offsets,
+                    const double* att_rot, const double* origin, const double step[3], const uint32_t counts[3],
+                    const double* rot_cov, const double* pos_cov, int iters, const double* rot_cov_tight,
+                    const double* pos_cov_tight, uint32_t k, double* rot_out, double* pos_out, double* sums_out,
+                    uint32_t* cand_out) {
+    if (!h) return LK_ERR_INVALID_ARG;
+    if (n_sets == 0) return LK_OK;
+    if (!pts || !set_offsets || !att_offsets || !att_rot || !origin || !step || !counts || !rot_cov || !pos_cov ||
+        !rot_cov_tight || !pos_cov_tight || !rot_out || !pos_out || !sums_out || !cand_out)
+        return fail(h, LK_ERR_INVALID_ARG, "null argument");
+    for (uint32_t s = 0; s < n_sets; ++s) {
+        if (set_offsets[s + 1] < set_offsets[s]) return fail(h, LK_ERR_INVALID_ARG, "set_offsets not monotone");
+        if (att_offsets[s + 1] < att_offsets[s]) return fail(h, LK_ERR_INVALID_ARG, "att_offsets not monotone");
+    }
+    if (!counts[0] || !counts[1] || !counts[2]) return fail(h, LK_ERR_INVALID_ARG, "a zero lattice count");
+    if (k == 0 || k > LK_SEARCH_MAX_K) return fail(h, LK_ERR_INVALID_ARG, "k outside 1 .. LK_SEARCH_MAX_K");
+    if (iters < 1) return fail(h, LK_ERR_INVALID_ARG, "iters < 1");
+    if (!all_finite(att_rot + 9 * (size_t)att_offsets[0], 9 * (size_t)(att_offsets[n_sets] - att_offsets[0])) ||
+        !all_finite(origin, 3 * (size_t)n_sets) || !all_finite(step, 3) || !all_finite(rot_cov, 9) ||
+        !all_finite(pos_cov, 9) || !all_finite(rot_cov_tight, 9) || !all_finite(pos_cov_tight, 9))
+        return fail(h, LK_ERR_INVALID_ARG, "non-finite attitude, origin, step or covariance");
+    for (uint32_t s = 0; s < n_sets; ++s) {  // attitudes x lattice, stopping once past 2^32 (no factor reaches 2^32)
+        uint64_t n = att_offsets[s + 1] - att_offsets[s];
+        for (int j = 0; j < 3 && n < (1ull << 32); ++j) n *= counts[j];
+        if (n >= (1ull << 32)) return fail(h, LK_ERR_INVALID_ARG, "a set with 2^32 or more candidates");
+        if (n < k) return fail(h, LK_ERR_INVALID_ARG, "a set with fewer than k candidates");
+    }
+    if (!h->map.ready()) return fail(h, LK_ERR_NOT_READY, "no map: call lk_map_upload or lk_map_build first");
+    enter(h);
+    return h->scorer.search(h->map, h->g, n_sets, pts, set_offsets, att_offsets, att_rot, origin, step, counts, rot_cov,
+                            pos_cov, iters, rot_cov_tight, pos_cov_tight, k, rot_out, pos_out, sums_out, cand_out, h->stream,
+                            h->err);
 }
 
 int lk_batch_run_range(lk_handle h, uint32_t first, uint32_t count, int iters, int update_map) {

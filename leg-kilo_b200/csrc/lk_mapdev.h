@@ -96,8 +96,8 @@ class MapInserter {
     DevBuf win_pts_, win_small_;
     PinnedBuf h_win_;
 };
-// lk_score.cu — lk_score_poses and lk_refine_poses (DESIGN §3.11, §3.12), one per handle. Its scratch is stream-ordered; no
-// call keeps its contents.
+// lk_score.cu — lk_score_poses, lk_refine_poses and lk_search_poses (DESIGN §3.11-3.13), one per handle. Its scratch is
+// stream-ordered; no call keeps its contents.
 class PoseScorer {
    public:
     // Behind the calls' argument checks (n_poses >= 1, a map): the records of every pose of pose_set (rot / pos per pose,
@@ -108,11 +108,23 @@ class PoseScorer {
             uint32_t n_poses, const uint32_t* pose_set, const double* rot, const double* pos, const double* rot_cov,
             const double* pos_cov, int iters, double* rot_out, double* pos_out, double* sums_out, cudaStream_t s,
             std::string& err);
+    // lk_search_poses behind its argument checks (n_sets >= 1, 1 <= k <= LK_SEARCH_MAX_K, every set with k to 2^32 - 1
+    // candidates, a map): the candidates of each set expanded, scored and kept (best k) on the device window by window,
+    // the kept ones refined, re-scored with the tight blocks and ranked. One host synchronisation.
+    int search(const MapDevHost& mh, const Globals& g, uint32_t n_sets, const float* pts, const uint32_t* set_offsets,
+               const uint32_t* att_offsets, const double* att_rot, const double* origin, const double* step,
+               const uint32_t* counts, const double* rot_cov, const double* pos_cov, int iters, const double* rot_cov_tight,
+               const double* pos_cov_tight, uint32_t k, double* rot_out, double* pos_out, double* sums_out,
+               uint32_t* cand_out, cudaStream_t s, std::string& err);
+    size_t device_bytes() const;  // device scratch held (both calls), lk_debug_read(h, 4, ...)
+    size_t host_bytes() const;    // page-locked staging held
 
    private:
-    // points, items | sums | ScanConst per pose (staged in h_, which also receives the read-back), the partial rows of one
-    // window, the records
+    // points, items | sums | ScanConst per pose (staged in h_, which also receives the read-back; search: then the ranked
+    // results), the partial rows of one window, the records
     DevBuf pts_, small_, partial_, out_;
+    // search: the per-set table and the attitudes; one window's candidate constants | sums | items; the running best keys
+    DevBuf sets_, win_, best_;
     PinnedBuf h_;
 };
 // lk_mapio.cu

@@ -176,6 +176,41 @@ class Core {
         return out;
     }
 
+    // lk_search_poses: per set, its attitudes (att_offsets) times one position lattice (counts, step, origin[s]) scored
+    // with rot_cov / pos_cov, the best k kept, refined by `iters` steps, re-scored with the tight blocks and ordered by the
+    // tight count, on the device. xyzw / set_offsets as scorePoses. rot / pos receive the k results of each set (entry
+    // s k + j), cand their candidate indices; returns their tight records (LK_SCORE_STRIDE doubles each, laid out as
+    // LK_SCORE_*).
+    std::vector<double> searchPoses(const std::vector<float>& xyzw, const std::vector<uint32_t>& set_offsets,
+                                    const std::vector<uint32_t>& att_offsets, const std::vector<Mat3D>& att,
+                                    const std::vector<Vec3D>& origin, const Vec3D& step, const uint32_t counts[3],
+                                    const Mat3D& rot_cov, const Mat3D& pos_cov, int iters, const Mat3D& rot_cov_tight,
+                                    const Mat3D& pos_cov_tight, uint32_t k, std::vector<Mat3D>& rot, std::vector<Vec3D>& pos,
+                                    std::vector<uint32_t>& cand) {
+        if (set_offsets.empty() || att_offsets.size() != set_offsets.size() || origin.size() + 1 != set_offsets.size() ||
+            att.size() < att_offsets.back())
+            throw std::invalid_argument("searchPoses: set_offsets / att_offsets of n_sets + 1 entries, one origin per set");
+        const size_t n_sets = origin.size(), n = n_sets * k;
+        std::vector<double> A(9 * att.size()), O(3 * n_sets), R(9 * n), p(3 * n), out(LK_SCORE_STRIDE * n);
+        for (size_t a = 0; a < att.size(); ++a) {
+            RowMat3 Ra = att[a];
+            std::memcpy(&A[9 * a], Ra.data(), 72);
+        }
+        for (size_t s = 0; s < n_sets; ++s) std::memcpy(&O[3 * s], origin[s].data(), 24);
+        RowMat3 Cr = rot_cov, Cp = pos_cov, Crt = rot_cov_tight, Cpt = pos_cov_tight;
+        cand.resize(n);
+        check(lk_search_poses(h_, (uint32_t)n_sets, xyzw.data(), set_offsets.data(), att_offsets.data(), A.data(), O.data(),
+                              step.data(), counts, Cr.data(), Cp.data(), iters, Crt.data(), Cpt.data(), k, R.data(), p.data(),
+                              out.data(), cand.data()));
+        rot.resize(n);
+        pos.resize(n);
+        for (size_t m = 0; m < n; ++m) {
+            rot[m] = Eigen::Map<const RowMat3>(&R[9 * m]);
+            pos[m] = Eigen::Map<const Vec3D>(&p[3 * m]);
+        }
+        return out;
+    }
+
     // VoxelMapManager::mapSliding (voxel_map.cc:552-571): drop the root voxels that left the +-half_map_size window.
     bool mapSliding(const Vec3D& position_last, uint64_t* removed = nullptr) {
         int32_t slid = 0;

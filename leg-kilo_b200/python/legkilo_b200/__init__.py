@@ -54,6 +54,7 @@ def lib():
         L.lk_map_insert.argtypes = [vp, u32, vp, vp, vp, vp, vp, vp]
         L.lk_score_poses.argtypes = [vp, u32, vp, vp, u32] + [vp] * 6
         L.lk_refine_poses.argtypes = [vp, u32, vp, vp, u32] + [vp] * 5 + [C.c_int] + [vp] * 3
+        L.lk_search_poses.argtypes = [vp, u32] + [vp] * 9 + [C.c_int, vp, vp, u32] + [vp] * 4
         L.lk_map_stats.argtypes = [vp, vp]
         L.lk_map_slide.argtypes = [vp, vp, vp, vp]
         L.lk_map_memory.argtypes = [vp, vp]
@@ -256,6 +257,42 @@ class Engine:
                                         _p(rot_cov), _p(pos_cov), int(iters), _p(rot_out), _p(pos_out),
                                         None if rec is None else _p(rec)))
         return rot_out, pos_out, rec
+
+    def search_poses(self, pts, set_offsets, att_offsets, att_rot, origin, step, counts, rot_cov, pos_cov, iters,
+                     rot_cov_tight, pos_cov_tight, k):
+        """lk_search_poses: per set, a lattice of candidate poses (its attitudes att_rot[att_offsets[s]:att_offsets[s + 1]]
+        times counts = (nx, ny, nz) positions spaced step from origin[s]) scored with rot_cov / pos_cov, the best k kept,
+        refined by `iters` steps, re-scored with rot_cov_tight / pos_cov_tight and ordered by that count, all on the
+        device. Returns (rot [n_sets, k, 3, 3], pos [n_sets, k, 3], tight records float64 [n_sets, k, 32], candidate
+        index uint32 [n_sets, k])."""
+        pts = np.ascontiguousarray(pts, np.float32).reshape(-1, 4)
+        so = np.ascontiguousarray(set_offsets, np.uint32).reshape(-1)
+        ao = np.ascontiguousarray(att_offsets, np.uint32).reshape(-1)
+        if len(so) < 1 or len(ao) != len(so):
+            raise ValueError("set_offsets and att_offsets need n_sets + 1 entries each")
+        if len(pts) < int(so[-1]):
+            raise ValueError(f"set_offsets ends at point {int(so[-1])}, pts has {len(pts)}")
+        n_sets = len(so) - 1
+        att = np.ascontiguousarray(att_rot, np.float64).reshape(-1, 9)
+        if len(att) < int(ao[-1]):
+            raise ValueError(f"att_offsets ends at attitude {int(ao[-1])}, att_rot has {len(att)}")
+        org = np.ascontiguousarray(origin, np.float64).reshape(n_sets, 3)
+        st = np.ascontiguousarray(step, np.float64).reshape(3)
+        cn = np.ascontiguousarray(counts, np.uint32).reshape(3)
+        covs = [np.ascontiguousarray(c, np.float64).reshape(9) for c in (rot_cov, pos_cov, rot_cov_tight, pos_cov_tight)]
+        k = int(k)
+        rot_out, pos_out = np.zeros((n_sets, k, 3, 3)), np.zeros((n_sets, k, 3))
+        rec, cand = np.zeros((n_sets, k, abi.SCORE_STRIDE)), np.zeros((n_sets, k), np.uint32)
+        self._chk(lib().lk_search_poses(self.h, n_sets, _p(pts), _p(so), _p(ao), _p(att), _p(org), _p(st), _p(cn),
+                                        _p(covs[0]), _p(covs[1]), int(iters), _p(covs[2]), _p(covs[3]), k, _p(rot_out),
+                                        _p(pos_out), _p(rec), _p(cand)))
+        return rot_out, pos_out, rec, cand
+
+    def scorer_scratch(self):
+        """lk_debug_read(h, 4): (device bytes, page-locked bytes) the pose scorer holds."""
+        out = np.zeros(2, np.uint64)
+        self._chk(lib().lk_debug_read(self.h, 4, _p(out), out.nbytes))
+        return int(out[0]), int(out[1])
 
     def map_slide(self, position):
         """VoxelMapManager::mapSliding (voxel_map.cc:552-571). Returns (slid, removed root voxels)."""
